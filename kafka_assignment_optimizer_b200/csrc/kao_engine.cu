@@ -17,6 +17,7 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 // The search kernels are instantiated in kao_inst.cu (one object per row width / counter depth /
@@ -211,7 +212,7 @@ struct kao_handle {
     int p2p_rank = 0, p2p_world = 1;
     uint64_t p2p_calls = 0;
     uint32_t patience = 0, last_rounds = 0;
-    unsigned long long *d_lkeys = nullptr; size_t lkeys_cap = 0;
+    unsigned long long *d_lkeys = nullptr;   // kMailRounds keys, sharded search only
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
 };
@@ -234,7 +235,7 @@ struct PersistArgs {
     unsigned long long *all_keys;
 };
 
-template <class Cfg> static cudaError_t set_smem_attr(kao_handle *h, const void *kern, bool *done)
+static cudaError_t set_smem_attr(kao_handle *h, const void *kern, bool *done)
 {
     if (!done[h->device & 63]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
@@ -250,7 +251,7 @@ struct LaunchRound {
         constexpr int T = threads_for<Cfg::W>();
         auto kern = search_round_kernel<Cfg, T>;
         static bool done[64] = {};
-        cudaError_t e = set_smem_attr<Cfg>(h, reinterpret_cast<const void *>(kern), done);
+        cudaError_t e = set_smem_attr(h, reinterpret_cast<const void *>(kern), done);
         if (e != cudaSuccess) return e;
         const uint32_t n = a.hi - a.lo, warps = T / 32;
         uint32_t grid = (n + warps - 1) / warps;
@@ -264,28 +265,38 @@ struct LaunchRound {
 template <bool kDelta> struct LaunchPersistent {
     template <class Cfg> cudaError_t run(kao_handle *h, const PersistArgs &a) const
     {
-        {
-            constexpr int T = kDelta ? KAO_THREADS_DELTA : cfg_threads<Cfg>();
-            auto kern = search_persistent_kernel<Cfg, T, kDelta>;
-            static bool done[64] = {};
-            cudaError_t e = set_smem_attr<Cfg>(h, reinterpret_cast<const void *>(kern), done);
-            if (e != cudaSuccess) return e;
-            Params prm = h->prm;
-            // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch)
-            SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF)
-                            : (kDelta && Cfg::W > 2) ? make_plan_delta_wide(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF) : h->plan;
-            if (plan.total > 227u * 1024u) return cudaErrorInvalidConfiguration;
-            uint64_t seed = a.seed; uint32_t fr = a.first_round, rounds = a.rounds, rs = a.round_size;
-            unsigned long long *keys = a.d_keys, *all = a.all_keys; unsigned int *bar = a.d_bar;
-            P2P pp = a.pp;
-            void *args[] = {&prm, &plan, &seed, &fr, &rounds, &rs, &keys, &bar, &pp, &all};
-            ++h->launches;
-            // cooperative launch: all CTAs are guaranteed co-resident, which the grid barrier needs
-            return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3(h->grid), dim3(T), args,
-                                               plan.total, a.st);
-        }
+        constexpr int T = kDelta ? KAO_THREADS_DELTA : cfg_threads<Cfg>();
+        auto kern = search_persistent_kernel<Cfg, T, kDelta>;
+        static bool done[64] = {};
+        cudaError_t e = set_smem_attr(h, reinterpret_cast<const void *>(kern), done);
+        if (e != cudaSuccess) return e;
+        Params prm = h->prm;
+        // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch)
+        SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF)
+                        : (kDelta && Cfg::W > 2) ? make_plan_delta_wide(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF) : h->plan;
+        if (plan.total > 227u * 1024u) return cudaErrorInvalidConfiguration;
+        uint64_t seed = a.seed; uint32_t fr = a.first_round, rounds = a.rounds, rs = a.round_size;
+        unsigned long long *keys = a.d_keys, *all = a.all_keys; unsigned int *bar = a.d_bar;
+        P2P pp = a.pp;
+        void *args[] = {&prm, &plan, &seed, &fr, &rounds, &rs, &keys, &bar, &pp, &all};
+        ++h->launches;
+        // cooperative launch: all CTAs are guaranteed co-resident, which the grid barrier needs
+        return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3(h->grid), dim3(T), args,
+                                           plan.total, a.st);
     }
 };
+
+// f(std::integral_constant<int, W>{}) for the session's row width W (32-bit words per row): the one place a
+// row width becomes a template argument
+template <class F> static decltype(auto) with_row_width(int W, F &&f)
+{
+    switch (W) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    default: return f(std::integral_constant<int, 8>{});
+    }
+}
 
 template <int W, int NPH, int kRack, class F, class A>
 static cudaError_t dispatch_obj(kao_handle *h, const F &f, const A &a)
@@ -307,12 +318,8 @@ static cudaError_t dispatch_w(kao_handle *h, const F &f, const A &a)
 }
 template <class F, class A> static cudaError_t dispatch(kao_handle *h, const F &f, const A &a)
 {
-    switch (h->hm.W) {                                    // one counter depth: per-lane column counts up to 255
-    case 1: return dispatch_w<1, 5>(h, f, a);
-    case 2: return dispatch_w<2, 5>(h, f, a);
-    case 4: return dispatch_w<4, 5>(h, f, a);
-    default: return dispatch_w<8, 5>(h, f, a);
-    }
+    // one counter depth: per-lane column counts up to 255
+    return with_row_width(h->hm.W, [&](auto w) { return dispatch_w<decltype(w)::value, 5>(h, f, a); });
 }
 // all rounds of a search in one cooperative launch, with the evaluator the session selected
 static cudaError_t launch_persistent(kao_handle *h, const PersistArgs &pa, bool delta)
@@ -342,12 +349,9 @@ static cudaError_t launch_round(kao_handle *h, uint64_t seed, uint32_t round, ui
 static cudaError_t launch_apply(kao_handle *h, uint64_t seed, uint32_t round, uint32_t round_size,
                                 const unsigned long long *d_key, int regen_only, cudaStream_t st)
 {
-    switch (h->hm.W) {
-    case 1: apply_winner_kernel<1><<<1, 1024, 0, st>>>(h->prm, seed, round, round_size, d_key, regen_only); break;
-    case 2: apply_winner_kernel<2><<<1, 1024, 0, st>>>(h->prm, seed, round, round_size, d_key, regen_only); break;
-    case 4: apply_winner_kernel<4><<<1, 1024, 0, st>>>(h->prm, seed, round, round_size, d_key, regen_only); break;
-    default: apply_winner_kernel<8><<<1, 1024, 0, st>>>(h->prm, seed, round, round_size, d_key, regen_only); break;
-    }
+    with_row_width(h->hm.W, [&](auto w) {
+        apply_winner_kernel<decltype(w)::value><<<1, 1024, 0, st>>>(h->prm, seed, round, round_size, d_key, regen_only);
+    });
     ++h->launches;
     return cudaGetLastError();
 }
@@ -375,6 +379,15 @@ static int destroy_impl(kao_handle *h)
     delete h;
     return KAO_OK;
 }
+
+// Owns a session; closing it keeps kao_last_error() on the failure that led there.
+struct HandleOwner {
+    kao_handle *h = nullptr;
+    HandleOwner() = default;
+    HandleOwner(const HandleOwner &) = delete;
+    ~HandleOwner() { close(); }
+    void close() { const std::string keep = g_err; destroy_impl(h); g_err = keep; h = nullptr; }
+};
 
 static int reset_impl(kao_handle *h)
 {
@@ -478,16 +491,11 @@ static int create_handle(const kao_problem *pb, int32_t device, kao_handle **out
 {
     if (!pb || !out) return fail(KAO_E_ARG, "null argument");
     *out = nullptr;
-    kao_handle *h = new kao_handle();
-    const int rc = create_impl(pb, device, h);
-    if (rc != KAO_OK) {
-        const std::string keep = g_err;
-        destroy_impl(h);
-        g_err = keep;
-        return rc;
-    }
-    *out = h;
-    return KAO_OK;
+    HandleOwner s;
+    s.h = new kao_handle();
+    const int rc = create_impl(pb, device, s.h);
+    if (rc == KAO_OK) { *out = s.h; s.h = nullptr; }
+    return rc;
 }
 
 static int set_base_impl(kao_handle *h, const int32_t *replicas)
@@ -503,12 +511,9 @@ static int eval_on_device(kao_handle *h, const uint32_t *d_bits, const uint8_t *
                           long long *d_viol, long long *d_obj)
 {
     const int blocks = (n * 32 + 255) / 256;
-    switch (h->hm.W) {
-    case 1: eval_batch_kernel<1, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj); break;
-    case 2: eval_batch_kernel<2, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj); break;
-    case 4: eval_batch_kernel<4, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj); break;
-    default: eval_batch_kernel<8, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj); break;
-    }
+    with_row_width(h->hm.W, [&](auto w) {
+        eval_batch_kernel<decltype(w)::value, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj);
+    });
     ++h->launches;
     CUDA_TRY(cudaGetLastError());
     return KAO_OK;
@@ -546,6 +551,15 @@ static bool delta_fits(const kao_handle *h)
     if (h->hm.W <= 2) return true;                              // the session's own plan (validated at kao_create)
     return make_plan_delta_wide(h->hm.W, h->hm.Ppad, KAO_THREADS_DELTA, h->hm.P, h->hm.RF).total <= 227u * 1024u;
 }
+// the arguments every search call checks (kao_search*, kao_candidate_keys*, kao_solve); kao_solve has no session
+// yet (h == nullptr): each of its sessions checks delta evaluation again when it searches
+static int check_search_args(const kao_handle *h, uint32_t rounds, uint32_t round_size, bool delta)
+{
+    if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
+    if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
+    if (delta && h && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
+    return KAO_OK;
+}
 
 static int reserve_keys(kao_handle *h, uint32_t rounds)
 {
@@ -573,24 +587,19 @@ static P2P solo_p2p(kao_handle *h, uint32_t idx_lo, uint32_t idx_hi)
     return pp;
 }
 
-static int search_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds,
-                       uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
+// A search call on a session around launch_rounds(), which enqueues its (at least one) rounds into h->d_keys: event
+// timing, the displaced lists in HBM rebuilt once at the end for the per-round entry points, the keys downloaded.
+template <class F>
+static int timed_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
+                        uint64_t *round_keys, double *device_ms, F &&launch_rounds)
 {
-    if (!h) return fail(KAO_E_ARG, "null handle");
-    if (delta && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
-    if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
-    if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
     CUDA_TRY(cudaSetDevice(h->device));
     h->last_rounds = 0;
     int rc = reserve_keys(h, rounds);
     if (rc != KAO_OK) return rc;
-    CUDA_TRY(cudaMemsetAsync(h->d_bar, 0, kBarBytes, 0));
     CUDA_TRY(cudaEventRecord(h->ev0, 0));
     if (rounds) {
-        // all rounds in one cooperative launch; the HBM base is kept current by CTA 0, the displaced
-        // lists in HBM are rebuilt once at the end for the per-round entry points
-        CUDA_TRY(launch_persistent(h, PersistArgs{seed, first_round, rounds, round_size, h->d_keys, h->d_bar, 0,
-                                                  solo_p2p(h, 0, round_size), nullptr}, delta));
+        if ((rc = launch_rounds()) != KAO_OK) return rc;
         CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
     }
     CUDA_TRY(cudaEventRecord(h->ev1, 0));
@@ -600,14 +609,29 @@ static int search_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint3
         CUDA_TRY(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
         *device_ms = ms;
     }
-    if (rounds) {
-        unsigned int st[4] = {0, 0, 0, 0};
-        CUDA_TRY(cudaMemcpy(st, h->d_bar, 16, cudaMemcpyDeviceToHost));
-        if (st[2]) return fail(KAO_E_CUDA, "search kernel timed out at a grid barrier");
-        h->last_rounds = st[3];
-    }
     if (round_keys && rounds)
         CUDA_TRY(cudaMemcpy(round_keys, h->d_keys, (size_t)rounds * 8, cudaMemcpyDeviceToHost));
+    return KAO_OK;
+}
+
+static int search_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds,
+                       uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
+{
+    if (!h) return fail(KAO_E_ARG, "null handle");
+    int rc = check_search_args(h, rounds, round_size, delta);
+    if (rc != KAO_OK) return rc;
+    rc = timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, [&]() -> int {
+        // all rounds in one cooperative launch; the HBM base is kept current by CTA 0
+        CUDA_TRY(cudaMemsetAsync(h->d_bar, 0, kBarBytes, 0));
+        CUDA_TRY(launch_persistent(h, PersistArgs{seed, first_round, rounds, round_size, h->d_keys, h->d_bar, 0,
+                                                  solo_p2p(h, 0, round_size), nullptr}, delta));
+        return KAO_OK;
+    });
+    if (rc != KAO_OK || !rounds) return rc;
+    unsigned int st[4] = {0, 0, 0, 0};
+    CUDA_TRY(cudaMemcpy(st, h->d_bar, 16, cudaMemcpyDeviceToHost));
+    if (st[2]) return fail(KAO_E_CUDA, "search kernel timed out at a grid barrier");
+    h->last_rounds = st[3];
     return KAO_OK;
 }
 
@@ -623,9 +647,9 @@ static int candidate_keys_impl(kao_handle *h, uint64_t seed, uint32_t round, uin
                                uint32_t idx_begin, uint32_t count, uint64_t *keys, bool delta)
 {
     if (!h || !keys) return fail(KAO_E_ARG, "null argument");
-    if (!check_round_args(round_size) || idx_begin > round_size || count > round_size - idx_begin)
-        return fail(KAO_E_ARG, "bad index range");
-    if (delta && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
+    const int rc = check_search_args(h, 1, round_size, delta);
+    if (rc != KAO_OK) return rc;
+    if (idx_begin > round_size || count > round_size - idx_begin) return fail(KAO_E_ARG, "bad index range");
     if (count == 0) return KAO_OK;
     CUDA_TRY(cudaSetDevice(h->device));
     DevTmp<unsigned long long> all;
@@ -657,6 +681,7 @@ static int ensure_mailbox(kao_handle *h)
 static int publish_mailboxes(kao_handle *h, int rank, int world)
 {
     if (!h->d_mailptrs) CUDA_TRY(dalloc(h, &h->d_mailptrs, sizeof(Mailbox *) * kMaxPeers));
+    if (!h->d_lkeys) CUDA_TRY(dalloc(h, &h->d_lkeys, (size_t)kMailRounds * 8));     // round keys of one launch
     CUDA_TRY(cudaMemcpy(h->d_mailptrs, h->peer_mail, sizeof(Mailbox *) * kMaxPeers, cudaMemcpyHostToDevice));
     h->p2p_rank = rank; h->p2p_world = world; h->p2p_calls = 0;
     return KAO_OK;
@@ -696,62 +721,45 @@ static int sharded_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint
                         uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
 {
     if (!h) return fail(KAO_E_ARG, "null handle");
-    if (delta && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
-    if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
-    if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
-    if (h->p2p_world < 2 || !h->peer_mail[h->p2p_world - 1]) return fail(KAO_E_STATE, "kao_p2p_connect first");
-    CUDA_TRY(cudaSetDevice(h->device));
-    h->last_rounds = 0;
-    int rc = reserve_keys(h, rounds);
+    const int rc = check_search_args(h, rounds, round_size, delta);
     if (rc != KAO_OK) return rc;
-    if (h->lkeys_cap < kMailRounds) {
-        CUDA_TRY(dalloc(h, &h->d_lkeys, (size_t)kMailRounds * 8));
-        h->lkeys_cap = kMailRounds;
-    }
+    if (h->p2p_world < 2 || !h->peer_mail[h->p2p_world - 1]) return fail(KAO_E_STATE, "kao_p2p_connect first");
     const int world = h->p2p_world, rank = h->p2p_rank;
     // contiguous slice of every round for this rank (same split on every rank)
     const uint32_t base = round_size / world, extra = round_size % world;
     const uint32_t lo = rank * base + ((uint32_t)rank < extra ? rank : extra);
     const uint32_t hi = lo + base + ((uint32_t)rank < extra ? 1 : 0);
-    unsigned long long best = kKeyNone;                             // early-stop state, carried from launch to launch
-    uint32_t stall = 0;
-    CUDA_TRY(cudaEventRecord(h->ev0, 0));
-    for (uint32_t done = 0; done < rounds; done += kMailRounds) {
-        const uint32_t n = rounds - done < kMailRounds ? rounds - done : kMailRounds;
-        const int bank = (int)(h->p2p_calls & 1);
-        ++h->p2p_calls;
-        // the OTHER bank is reset now: no peer can reach the next launch before this rank has taken
-        // part in every round of this one (docs/MODEL.md §7), so the reset cannot race with a writer
-        CUDA_TRY(cudaMemsetAsync(&h->d_mail->slot[bank ^ 1][0][0], 0xFF, sizeof(h->d_mail->slot[0]), 0));
-        fill_u64_kernel<<<32, 256>>>(h->d_lkeys, kKeyNone, (size_t)n);
-        CUDA_TRY(cudaMemsetAsync(h->d_bar, 0, kBarBytes, 0));
-        h->launches += 1;
-        P2P pp = solo_p2p(h, lo, hi);
-        pp.rank = rank; pp.world = world; pp.bank = bank;
-        pp.mail = h->d_mailptrs;
-        pp.lkeys = h->d_lkeys; pp.release = h->d_bar + 1;
-        pp.best_in = best; pp.stall_in = stall;
-        const PersistArgs pa{seed, first_round + done, n, round_size, h->d_keys + done, h->d_bar, 0, pp, nullptr};
-        CUDA_TRY(launch_persistent(h, pa, delta));
-        unsigned int st[8] = {};
-        CUDA_TRY(cudaMemcpy(st, h->d_bar, kBarBytes, cudaMemcpyDeviceToHost));
-        if (st[2]) return fail(KAO_E_CUDA, "sharded search timed out waiting for a peer GPU");
-        h->last_rounds = done + st[3];
-        std::memcpy(&best, st + 4, 8);
-        { unsigned long long s64; std::memcpy(&s64, st + 6, 8); stall = (uint32_t)s64; }
-        if (st[3] < n) break;                                   // early stop (every rank stops at the same round)
-    }
-    if (rounds) CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
-    CUDA_TRY(cudaEventRecord(h->ev1, 0));
-    CUDA_TRY(cudaEventSynchronize(h->ev1));
-    if (device_ms) {
-        float ms = 0;
-        CUDA_TRY(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-        *device_ms = ms;
-    }
-    if (round_keys && rounds)
-        CUDA_TRY(cudaMemcpy(round_keys, h->d_keys, (size_t)rounds * 8, cudaMemcpyDeviceToHost));
-    return KAO_OK;
+    // one cooperative launch per kMailRounds rounds: the mailbox bank alternates from launch to launch
+    return timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, [&]() -> int {
+        unsigned long long best = kKeyNone;                         // early-stop state, carried from launch to launch
+        uint32_t stall = 0;
+        for (uint32_t done = 0; done < rounds; done += kMailRounds) {
+            const uint32_t n = rounds - done < kMailRounds ? rounds - done : kMailRounds;
+            const int bank = (int)(h->p2p_calls & 1);
+            ++h->p2p_calls;
+            // the OTHER bank is reset now: no peer can reach the next launch before this rank has taken
+            // part in every round of this one (docs/MODEL.md §7), so the reset cannot race with a writer
+            CUDA_TRY(cudaMemsetAsync(&h->d_mail->slot[bank ^ 1][0][0], 0xFF, sizeof(h->d_mail->slot[0]), 0));
+            fill_u64_kernel<<<32, 256>>>(h->d_lkeys, kKeyNone, (size_t)n);
+            CUDA_TRY(cudaMemsetAsync(h->d_bar, 0, kBarBytes, 0));
+            h->launches += 1;
+            P2P pp = solo_p2p(h, lo, hi);
+            pp.rank = rank; pp.world = world; pp.bank = bank;
+            pp.mail = h->d_mailptrs;
+            pp.lkeys = h->d_lkeys; pp.release = h->d_bar + 1;
+            pp.best_in = best; pp.stall_in = stall;
+            const PersistArgs pa{seed, first_round + done, n, round_size, h->d_keys + done, h->d_bar, 0, pp, nullptr};
+            CUDA_TRY(launch_persistent(h, pa, delta));
+            unsigned int st[8] = {};
+            CUDA_TRY(cudaMemcpy(st, h->d_bar, kBarBytes, cudaMemcpyDeviceToHost));
+            if (st[2]) return fail(KAO_E_CUDA, "sharded search timed out waiting for a peer GPU");
+            h->last_rounds = done + st[3];
+            std::memcpy(&best, st + 4, 8);
+            { unsigned long long s64; std::memcpy(&s64, st + 6, 8); stall = (uint32_t)s64; }
+            if (st[3] < n) break;                                   // early stop (every rank stops at the same round)
+        }
+        return KAO_OK;
+    });
 }
 
 static int profile_rounds_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds,
@@ -793,10 +801,10 @@ static int eval_impl(const kao_problem *pb, int32_t device, const int32_t *repli
                      int64_t *violation, int64_t *objective)
 {
     if (!pb || !replicas || n < 0 || !violation || !objective) return fail(KAO_E_ARG, "bad argument");
-    kao_handle *h = nullptr;
-    int rc = create_handle(pb, device, &h);
+    HandleOwner s;
+    int rc = create_handle(pb, device, &s.h);
     if (rc != KAO_OK) return rc;
-    struct Closer { kao_handle *h; ~Closer() { const std::string keep = g_err; destroy_impl(h); g_err = keep; } } closer{h};
+    kao_handle *h = s.h;
     const HostModel &m = h->hm;
     const size_t nb = (size_t)m.W * m.Ppad, nl = (size_t)m.Ppad;
     if (n == 0) return KAO_OK;
@@ -886,30 +894,89 @@ static int enable_peers(int dev, const std::vector<int> &devs)
     return KAO_OK;
 }
 
-struct GangResult {                                   // what rank 0 reports per restart
+// ---- what both kao_solve drivers (restarts, sharded rounds) share
+// KAO_TRACE (stderr): where a kao_solve call spends its host time
+static void stamp(std::chrono::steady_clock::time_point t0, const char *what)
+{
+    static const bool trace = std::getenv("KAO_TRACE") != nullptr;
+    if (trace)
+        std::fprintf(stderr, "[kao trace] kao_solve: %s at %.3f ms\n", what,
+                     std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+}
+
+// the kao_options flags that configure a session: KAO_FLAG_PATIENCE(n), and KAO_FLAG_ROW_MAJOR (the column-major
+// evaluator is the default where the layout allows it; the flag selects the other full evaluator, same keys)
+static void apply_options(kao_handle *h, const kao_options *opt)
+{
+    h->patience = opt->flags >> 16;
+    if (opt->flags & KAO_FLAG_ROW_MAJOR) h->evaluator = KAO_EVAL_ROW_MAJOR;
+}
+
+struct Outcome {                                      // the final assignment of one restart
     int64_t viol = 0, obj = 0;
     int32_t moves = 0;
-    uint32_t rounds = 0;
-    double dev_ms = 0;
+    uint32_t restart = 0;
+    uint64_t key = kKeyNone;                          // its last round key
+    std::vector<int32_t> reps;
 };
+// the restart kao_solve returns: lowest violation, then highest objective, then lowest restart index
+static bool better(const Outcome &a, const Outcome &b)
+{
+    if (a.viol != b.viol) return a.viol < b.viol;
+    if (a.obj != b.obj) return a.obj > b.obj;
+    return a.restart < b.restart;
+}
+// the session's base after restart r, whose round keys the search wrote to keys
+static int read_outcome(kao_handle *h, uint32_t r, const std::vector<uint64_t> &keys, Outcome &o)
+{
+    o.reps.resize((size_t)h->hm.P * h->hm.RF);
+    o.restart = r;
+    o.key = h->last_rounds ? keys[h->last_rounds - 1] : kKeyNone;
+    return get_base_impl(h, o.reps.data(), &o.viol, &o.obj, &o.moves);
+}
+struct Solved {                                       // what a kao_solve driver hands back
+    Outcome win;
+    uint32_t rounds_run = 0;                          // summed over the restarts
+    double dev_ms = 0;                                // summed over the restarts of a GPU, max over the GPUs
+    HostModel hm;                                     // GPU 0's
+};
+// worker(i) for each GPU of the call, GPU 0 on the calling thread and one host thread for every other; a failure is
+// reported with its GPU named when there are several
+template <class F> static int on_each_gpu(const std::vector<int> &devs, F &&worker)
+{
+    const int world = (int)devs.size();
+    std::vector<int> rcs(world, KAO_OK);
+    std::vector<std::string> errs(world);
+    auto run = [&](int i) {
+        rcs[i] = guarded([&] { return worker(i); });
+        if (rcs[i] != KAO_OK) errs[i] = g_err;
+    };
+    std::vector<std::thread> th;
+    for (int i = 1; i < world; ++i) th.emplace_back(run, i);
+    run(0);
+    for (auto &t : th) t.join();
+    for (int i = 0; i < world; ++i)
+        if (rcs[i] != KAO_OK) return fail(rcs[i], world > 1 ? "GPU " + std::to_string(devs[i]) + ": " + errs[i] : errs[i]);
+    return KAO_OK;
+}
 
-static int solve_gang(const kao_problem *pb, const kao_options *opt, kao_result *res, const std::vector<int> &devs,
-                      uint32_t restarts, bool delta, std::vector<uint64_t> &keys, std::vector<int32_t> &reps,
-                      uint32_t &rounds_run, double &dev_ms_total, HostModel &hm_out)
+// The rounds of every restart sharded over the GPUs: every round's index range is split between them and its winner
+// agreed through the mailboxes, so all GPUs hold the same base.
+static int solve_gang(const kao_problem *pb, const kao_options *opt, const std::vector<int> &devs, uint32_t restarts,
+                      bool delta, Solved &out)
 {
     const int world = (int)devs.size();
     std::vector<kao_handle *> hs(world, nullptr);
-    std::vector<int> rcs(world, KAO_OK);
-    std::vector<std::string> errs(world);
     std::vector<double> ms(world, 0.0);
+    std::vector<uint64_t> keys(opt->rounds ? opt->rounds : 1, kKeyNone);
     Rendezvous meet(world);
-    bool have = false;
     static const bool trace = std::getenv("KAO_TRACE") != nullptr;       // stderr: where a multi-GPU solve spends its host time
     const auto t_start = std::chrono::steady_clock::now();
-    auto worker = [&](int i) {
-        int phase = 0;
+    return on_each_gpu(devs, [&](int i) {
+        int phase = 0, first = KAO_OK;                // this rank's first failure
+        std::string err;
         auto step = [&](int rc) {                     // record the first failure of this rank, then meet the others
-            if (rc != KAO_OK && rcs[i] == KAO_OK) { rcs[i] = rc; errs[i] = g_err; }
+            if (rc != KAO_OK && first == KAO_OK) { first = rc; err = g_err; }
             const auto t_a = std::chrono::steady_clock::now();
             const bool all_ok = meet.arrive(rc == KAO_OK);
             if (trace) {
@@ -921,8 +988,9 @@ static int solve_gang(const kao_problem *pb, const kao_options *opt, kao_result 
             ++phase;
             return all_ok;
         };
-        kao_handle *h = nullptr;
-        bool ok = step(guarded([&] { return create_handle(pb, devs[i], &h); }));
+        HandleOwner s;
+        bool ok = step(guarded([&] { return create_handle(pb, devs[i], &s.h); }));
+        kao_handle *h = s.h;
         hs[i] = h;
         if (ok) ok = step(guarded([&] {
             int rc = enable_peers(devs[i], devs);
@@ -931,14 +999,14 @@ static int solve_gang(const kao_problem *pb, const kao_options *opt, kao_result 
             h->mail_pooled = true;
             CUDA_TRY(cudaMemsetAsync(h->d_mail, 0xFF, sizeof(Mailbox), 0));   // kMailEmpty everywhere, before any peer can write
             CUDA_TRY(cudaStreamSynchronize(0));
-            h->patience = opt->flags >> 16;                         // KAO_FLAG_PATIENCE(n)
-            if (opt->flags & KAO_FLAG_ROW_MAJOR) h->evaluator = KAO_EVAL_ROW_MAJOR;
+            apply_options(h, opt);
             return KAO_OK;
         }));
         if (ok) ok = step(guarded([&] {
             for (int j = 0; j < world; ++j) h->peer_mail[j] = hs[j]->d_mail;    // unified addressing: a peer's pointer is valid here
             return publish_mailboxes(h, i, world);
         }));
+        Outcome cur;
         for (uint32_t r = 0; ok && r < restarts; ++r) {
             const uint64_t seed = opt->seed + 0x9E3779B97F4A7C15ull * r;
             ok = step(guarded([&] {
@@ -947,189 +1015,106 @@ static int solve_gang(const kao_problem *pb, const kao_options *opt, kao_result 
                 return rc;
             }));
             if (ok && i == 0) {                       // all ranks hold the same base: rank 0 reports it
-                GangResult g;
-                int rc = guarded([&] { return get_base_impl(h, reps.data(), &g.viol, &g.obj, &g.moves); });
-                if (rc == KAO_OK) {
-                    for (int j = 0; j < world; ++j) g.dev_ms = ms[j] > g.dev_ms ? ms[j] : g.dev_ms;
-                    dev_ms_total += g.dev_ms;
-                    rounds_run += h->last_rounds;
-                    if (!have || g.viol < res->violation || (g.viol == res->violation && g.obj > res->objective)) {
-                        std::memcpy(res->replicas, reps.data(), reps.size() * 4);
-                        res->violation = g.viol; res->objective = g.obj; res->moves = g.moves;
-                        res->key = h->last_rounds ? keys[h->last_rounds - 1] : kKeyNone;
-                        have = true;
-                    }
-                } else { rcs[0] = rc; errs[0] = g_err; }
+                const int rc = guarded([&] {
+                    const int rc = read_outcome(h, r, keys, cur);
+                    if (rc != KAO_OK) return rc;
+                    double dev_ms = 0;
+                    for (int j = 0; j < world; ++j) dev_ms = ms[j] > dev_ms ? ms[j] : dev_ms;
+                    out.dev_ms += dev_ms;
+                    out.rounds_run += h->last_rounds;
+                    if (r == 0 || better(cur, out.win)) out.win = cur;
+                    return KAO_OK;
+                });
+                if (rc != KAO_OK) { first = rc; err = g_err; }
             }
-            if (ok) ok = meet.arrive(i != 0 || rcs[0] == KAO_OK);   // nobody resets the base while rank 0 reads it
+            if (ok) ok = meet.arrive(first == KAO_OK);   // nobody resets the base while rank 0 reads it
         }
-        if (i == 0 && h) hm_out = h->hm;
-        if (h) { const std::string keep = g_err; destroy_impl(h); g_err = keep; }
+        if (i == 0 && h) out.hm = h->hm;
+        s.close();
         if (trace)
             std::fprintf(stderr, "[kao trace] gpu %d destroyed at %.3f ms\n", devs[i],
                          std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count());
-    };
-    std::vector<std::thread> th;
-    for (int i = 1; i < world; ++i) th.emplace_back(worker, i);
-    worker(0);
-    for (auto &t : th) t.join();
-    for (int i = 0; i < world; ++i)
-        if (rcs[i] != KAO_OK) return fail(rcs[i], "GPU " + std::to_string(devs[i]) + ": " + errs[i]);
-    return KAO_OK;
+        return first == KAO_OK ? KAO_OK : fail(first, err);
+    });
 }
 
-// KAO_FLAG_SPREAD_RESTARTS: the restarts of one kao_solve side by side on the GPUs of the call — restart r runs on
-// GPU r mod N as an ordinary single-GPU search (no exchange between the GPUs at all), one host thread per GPU; the
-// best final assignment wins, ties go to the lowest restart index: exactly what one GPU returns for the same call.
-static int solve_spread(const kao_problem *pb, const kao_options *opt, kao_result *res, const std::vector<int> &devs,
-                        uint32_t restarts, bool delta, uint32_t &rounds_run, double &dev_ms_total, HostModel &hm_out)
+// The restarts side by side on the GPUs of the call: restart r runs on GPU r mod N as an ordinary single-GPU search
+// (no exchange between the GPUs at all), one host thread per GPU and none for one GPU.  The winner is exactly what
+// one GPU returns for the same call: this is kao_solve on one GPU, and with KAO_FLAG_SPREAD_RESTARTS on several.
+static int solve_restarts(const kao_problem *pb, const kao_options *opt, const std::vector<int> &devs, uint32_t restarts,
+                          bool delta, std::chrono::steady_clock::time_point t0, Solved &out)
 {
     const int world = (int)devs.size();
-    struct Best {
-        bool have = false;
-        int64_t viol = 0, obj = 0;
-        int32_t moves = 0;
-        uint32_t restart = 0, rounds = 0;
-        uint64_t key = kKeyNone;
-        double dev_ms = 0;
-        std::vector<int32_t> reps;
-        HostModel hm;
-    };
-    std::vector<Best> best(world);
-    std::vector<int> rcs(world, KAO_OK);
-    std::vector<std::string> errs(world);
-    auto worker = [&](int i) {
-        Best &b = best[i];
-        rcs[i] = guarded([&]() -> int {
-            kao_handle *h = nullptr;
-            int rc = create_handle(pb, devs[i], &h);
+    std::vector<Solved> per(world);
+    const int rc = on_each_gpu(devs, [&](int i) {
+        Solved &g = per[i];
+        HandleOwner s;
+        int rc = create_handle(pb, devs[i], &s.h);
+        if (rc != KAO_OK) return rc;
+        stamp(t0, "session created (model built, tables uploaded, initial base)");
+        kao_handle *h = s.h;
+        apply_options(h, opt);
+        if (i == 0) g.hm = h->hm;
+        std::vector<uint64_t> keys(opt->rounds ? opt->rounds : 1, kKeyNone);
+        Outcome cur;
+        for (uint32_t r = (uint32_t)i; r < restarts; r += (uint32_t)world) {
+            double dev_ms = 0;
+            if (r != (uint32_t)i && (rc = reset_impl(h)) != KAO_OK) return rc;
+            rc = search_impl(h, opt->seed + 0x9E3779B97F4A7C15ull * r, 0, opt->rounds, opt->round_size, keys.data(), &dev_ms, delta);
             if (rc != KAO_OK) return rc;
-            struct Closer { kao_handle *h; ~Closer() { const std::string keep = g_err; destroy_impl(h); g_err = keep; } } closer{h};
-            h->patience = opt->flags >> 16;
-            if (opt->flags & KAO_FLAG_ROW_MAJOR) h->evaluator = KAO_EVAL_ROW_MAJOR;
-            b.hm = h->hm;
-            std::vector<uint64_t> keys(opt->rounds ? opt->rounds : 1, kKeyNone);
-            std::vector<int32_t> reps((size_t)pb->P * pb->RF);
-            bool first = true;
-            for (uint32_t r = (uint32_t)i; r < restarts; r += (uint32_t)world) {
-                double dev_ms = 0;
-                if (!first && (rc = reset_impl(h)) != KAO_OK) return rc;
-                first = false;
-                rc = search_impl(h, opt->seed + 0x9E3779B97F4A7C15ull * r, 0, opt->rounds, opt->round_size, keys.data(), &dev_ms, delta);
-                if (rc != KAO_OK) return rc;
-                int64_t viol = 0, obj = 0;
-                int32_t moves = 0;
-                rc = get_base_impl(h, reps.data(), &viol, &obj, &moves);
-                if (rc != KAO_OK) return rc;
-                b.dev_ms += dev_ms;
-                b.rounds += h->last_rounds;
-                if (!b.have || viol < b.viol || (viol == b.viol && obj > b.obj)) {
-                    b.have = true; b.viol = viol; b.obj = obj; b.moves = moves; b.restart = r;
-                    b.key = h->last_rounds ? keys[h->last_rounds - 1] : kKeyNone;
-                    b.reps = reps;
-                }
-            }
-            return KAO_OK;
-        });
-        if (rcs[i] != KAO_OK) errs[i] = g_err;
-    };
-    std::vector<std::thread> th;
-    for (int i = 1; i < world; ++i) th.emplace_back(worker, i);
-    worker(0);
-    for (auto &t : th) t.join();
-    for (int i = 0; i < world; ++i)
-        if (rcs[i] != KAO_OK) return fail(rcs[i], "GPU " + std::to_string(devs[i]) + ": " + errs[i]);
-    const Best *win = nullptr;
-    for (const Best &b : best) {
-        if (!b.have) continue;                        // more GPUs than restarts
-        rounds_run += b.rounds;
-        dev_ms_total = b.dev_ms > dev_ms_total ? b.dev_ms : dev_ms_total;
-        if (!win || b.viol < win->viol || (b.viol == win->viol && (b.obj > win->obj || (b.obj == win->obj && b.restart < win->restart)))) win = &b;
+            stamp(t0, "search done");
+            if ((rc = read_outcome(h, r, keys, cur)) != KAO_OK) return rc;
+            stamp(t0, "result downloaded and evaluated");
+            g.dev_ms += dev_ms;
+            g.rounds_run += h->last_rounds;
+            if (r == (uint32_t)i || better(cur, g.win)) g.win = cur;
+        }
+        return KAO_OK;
+    });
+    if (rc != KAO_OK) return rc;
+    out = std::move(per[0]);
+    for (int i = 1; i < world && (uint32_t)i < restarts; ++i) {     // a GPU past the number of restarts ran none
+        out.rounds_run += per[i].rounds_run;
+        out.dev_ms = per[i].dev_ms > out.dev_ms ? per[i].dev_ms : out.dev_ms;
+        if (better(per[i].win, out.win)) out.win = std::move(per[i].win);
     }
-    if (!win) return fail(KAO_E_STATE, "no restart ran");
-    std::memcpy(res->replicas, win->reps.data(), win->reps.size() * 4);
-    res->violation = win->viol; res->objective = win->obj; res->moves = win->moves; res->key = win->key;
-    hm_out = best[0].hm;
     return KAO_OK;
 }
 
 static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result *res)
 {
     if (!pb || !opt || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
-    if (opt->rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20)");
-    if (!check_round_args(opt->round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
+    int rc = check_search_args(nullptr, opt->rounds, opt->round_size, false);
+    if (rc != KAO_OK) return rc;
     const auto t0 = std::chrono::steady_clock::now();
     std::vector<int> devs;
-    int rc = pick_devices(opt, devs);
+    rc = pick_devices(opt, devs);
     if (rc != KAO_OK) return rc;
     const int world = (int)devs.size();
     // independent restarts (flags & 0xFF, 0 and 1 both mean a single search): each restarts from the
-    // initial base with its own seed; the best final assignment wins (violation, then objective)
+    // initial base with its own seed; the best final assignment wins (better())
     const uint32_t restarts = (opt->flags & 0xFFu) ? (opt->flags & 0xFFu) : 1u;
     const bool delta = (opt->flags & KAO_FLAG_DELTA) != 0;
-    uint32_t rounds_run = 0;
-    std::vector<uint64_t> keys(opt->rounds ? opt->rounds : 1, kKeyNone);
-    std::vector<int32_t> reps((size_t)pb->P * pb->RF);
-    double dev_ms_total = 0;
-    HostModel hm;
-    static const bool trace = std::getenv("KAO_TRACE") != nullptr;
-    auto stamp = [&](const char *what) {
-        if (trace)
-            std::fprintf(stderr, "[kao trace] kao_solve: %s at %.3f ms\n", what,
-                         std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
-    };
-    if (world == 1) {
-        kao_handle *h0 = nullptr;
-        rc = create_handle(pb, devs[0], &h0);
-        if (rc != KAO_OK) return rc;
-        stamp("session created (model built, tables uploaded, initial base)");
-        struct Closer { kao_handle *h; ~Closer() { const std::string keep = g_err; destroy_impl(h); g_err = keep; } } closer{h0};
-        h0->patience = opt->flags >> 16;                         // KAO_FLAG_PATIENCE(n)
-        // the column-major evaluator is the default where the layout allows it; the flag selects the other full evaluator (same keys)
-        if (opt->flags & KAO_FLAG_ROW_MAJOR) h0->evaluator = KAO_EVAL_ROW_MAJOR;
-        bool have = false;
-        for (uint32_t r = 0; r < restarts; ++r) {
-            double dev_ms = 0;
-            if (r && (rc = reset_impl(h0)) != KAO_OK) return rc;
-            rc = search_impl(h0, opt->seed + 0x9E3779B97F4A7C15ull * r, 0, opt->rounds, opt->round_size, keys.data(), &dev_ms, delta);
-            if (rc != KAO_OK) return rc;
-            stamp("search done");
-            int64_t viol = 0, obj = 0;
-            int32_t moves = 0;
-            rc = get_base_impl(h0, reps.data(), &viol, &obj, &moves);
-            if (rc != KAO_OK) return rc;
-            stamp("result downloaded and evaluated");
-            dev_ms_total += dev_ms;
-            rounds_run += h0->last_rounds;
-            if (!have || viol < res->violation || (viol == res->violation && obj > res->objective)) {
-                std::memcpy(res->replicas, reps.data(), reps.size() * 4);
-                res->violation = viol; res->objective = obj; res->moves = moves;
-                res->key = h0->last_rounds ? keys[h0->last_rounds - 1] : kKeyNone;
-                have = true;
-            }
-        }
-        hm = h0->hm;
-    } else if (opt->flags & KAO_FLAG_SPREAD_RESTARTS) {
-        rc = solve_spread(pb, opt, res, devs, restarts, delta, rounds_run, dev_ms_total, hm);
-        if (rc != KAO_OK) return rc;
-    } else {
-        rc = solve_gang(pb, opt, res, devs, restarts, delta, keys, reps, rounds_run, dev_ms_total, hm);
-        if (rc != KAO_OK) return rc;
-    }
-    stamp("session destroyed");
+    Solved s;
+    rc = world > 1 && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS) ? solve_gang(pb, opt, devs, restarts, delta, s)
+                                                                : solve_restarts(pb, opt, devs, restarts, delta, t0, s);
+    if (rc != KAO_OK) return rc;
+    stamp(t0, "session destroyed");
+    std::memcpy(res->replicas, s.win.reps.data(), s.win.reps.size() * 4);
+    res->violation = s.win.viol; res->objective = s.win.obj; res->moves = s.win.moves; res->key = s.win.key;
     res->feasible = res->violation == 0;
-    res->n_candidates = (uint64_t)rounds_run * opt->round_size;
-    res->rounds_run = rounds_run;
+    res->n_candidates = (uint64_t)s.rounds_run * opt->round_size;
+    res->rounds_run = s.rounds_run;
     res->restarts = restarts;
-    res->device_ms = dev_ms_total;
-    res->objective_bound = objective_upper_bound(hm, *pb);
+    res->device_ms = s.dev_ms;
+    res->objective_bound = objective_upper_bound(s.hm, *pb);
     if ((opt->flags & KAO_FLAG_BOUND) && res->feasible)
-        res->objective_bound = objective_flow_bound(hm, *pb, res->replicas, res->objective_bound);
+        res->objective_bound = objective_flow_bound(s.hm, *pb, res->replicas, res->objective_bound);
     res->optimal = res->feasible && res->objective == res->objective_bound;
-    res->key_obj_bits = hm.key_obj_bits;
+    res->key_obj_bits = s.hm.key_obj_bits;
     res->n_gpus = world;
     res->reserved = 0;
-    stamp("bound computed");
+    stamp(t0, "bound computed");
     res->total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (!res->feasible) { g_err = "no candidate satisfying C1..C7 was found"; return KAO_INFEASIBLE; }
     return KAO_OK;
