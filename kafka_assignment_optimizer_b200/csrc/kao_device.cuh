@@ -590,6 +590,11 @@ template <int W, int NPH> struct ColCounter {
     }
 };
 
+// High planes a per-lane column counter needs.  A lane takes 4 consecutive rows of every 128-row tile, so it
+// holds Ppad / 32 rows and one column of it can count that many: NPH 5 counts up to 255 (Ppad <= 7936), the
+// largest padding (8192 rows, P 7937..8160) needs a sixth plane.
+__host__ __device__ constexpr int counter_nph(int Ppad) { return Ppad / 32 > 255 ? 6 : 5; }
+
 __device__ __forceinline__ uint32_t bytecounts(uint32_t x)
 {
     uint32_t c = x - ((x >> 1) & 0x55555555u);
@@ -723,16 +728,18 @@ __device__ __forceinline__ int row_rack_terms(const uint32_t (&x)[W], int log2S_
     return abs(n - RF) + pen;
 }
 
-constexpr int kPlanes = 13;                 // 8 per-lane planes + 5 butterfly steps: counts < 8192
+// bit planes of a column count after the warp sum: 3 + NPH per-lane planes + 5 butterfly steps (NPH 5: counts
+// < 8192, NPH 6: < 16384)
+template <int NPH> constexpr int kPlanes = 3 + NPH + 5;
 
 template <int W, int NPH>
-__device__ __forceinline__ void load_planes(uint32_t (&pl)[kPlanes], const ColCounter<W, NPH> &c, int t)
+__device__ __forceinline__ void load_planes(uint32_t (&pl)[kPlanes<NPH>], const ColCounter<W, NPH> &c, int t)
 {
     pl[0] = c.ones[t]; pl[1] = c.twos[t]; pl[2] = c.fours[t];
 #pragma unroll
     for (int k = 0; k < NPH; ++k) pl[3 + k] = c.hi[k][t];
 #pragma unroll
-    for (int k = 3 + NPH; k < kPlanes; ++k) pl[k] = 0;
+    for (int k = 3 + NPH; k < kPlanes<NPH>; ++k) pl[k] = 0;
 }
 
 // C3 / C4 / C6: broker columns.  pl[i] = bit-sliced per-lane counts of NI 32-column items (items
@@ -743,11 +750,10 @@ __device__ __forceinline__ void load_planes(uint32_t (&pl)[kPlanes], const ColCo
 // one rack (NI <= S), so the rack totals of C6 are a segmented warp sum of the replica columns.
 // Returns this lane's share of the violation.
 template <int NI, int NP0>
-__device__ __forceinline__ int column_violation(uint32_t (&pl)[NI][kPlanes], int lane, int nA,
+__device__ __forceinline__ int column_violation(uint32_t (&pl)[NI][NP0 + 5], int lane, int nA,
                                                 const uint32_t *bndA, const uint32_t *bndB,
                                                 bool racks, int lead_mode, int log2S, int R, const Consts *cs)
 {
-    static_assert(NP0 + 5 <= kPlanes, "plane budget");
     int item = 0;
 #pragma unroll
     for (int step = 0; step < 5; ++step) {
@@ -1088,7 +1094,7 @@ __device__ void eval_candidate(const Params &d, const uint32_t *bitsT, const uin
     constexpr int NP0 = 3 + NPH;
     if constexpr (W <= 2) {
         // both counter sets in one pass: items 0..W-1 replica words, W..2W-1 leader words
-        uint32_t pl[2 * W][kPlanes];
+        uint32_t pl[2 * W][kPlanes<NPH>];
 #pragma unroll
         for (int t = 0; t < W; ++t) {
             load_planes<W, NPH>(pl[t], rc, t);
@@ -1096,7 +1102,7 @@ __device__ void eval_candidate(const Params &d, const uint32_t *bitsT, const uin
         }
         viol += column_violation<2 * W, NP0>(pl, lane, W, cs->bnd_rep, cs->bnd_ldr, true, 1, d.log2S, d.R, cs);
     } else {
-        uint32_t pl[W][kPlanes];
+        uint32_t pl[W][kPlanes<NPH>];
 #pragma unroll
         for (int t = 0; t < W; ++t) load_planes<W, NPH>(pl[t], rc, t);
         viol += column_violation<W, NP0>(pl, lane, W, cs->bnd_rep, cs->bnd_rep, true, 0, d.log2S, d.R, cs);

@@ -30,6 +30,8 @@ KAO_FOR_CFGS_NARROW(KAO_DECL_FULL, 1, 5) KAO_FOR_CFGS_NARROW(KAO_DECL_FULL, 2, 5
 KAO_FOR_CFGS_WIDE(KAO_DECL_FULL, 4, 5) KAO_FOR_CFGS_WIDE(KAO_DECL_FULL, 8, 5)
 KAO_FOR_CFGS_NARROW(KAO_DECL_DELTA, 1, 5) KAO_FOR_CFGS_NARROW(KAO_DECL_DELTA, 2, 5)
 KAO_FOR_CFGS_WIDE(KAO_DECL_DELTA, 4, 5) KAO_FOR_CFGS_WIDE(KAO_DECL_DELTA, 8, 5)
+// the deeper column counters of 8192 padded rows (counter_nph): only one-word rows fit shared memory there
+KAO_FOR_CFGS_NARROW(KAO_DECL_FULL, 1, 6) KAO_FOR_CFGS_NARROW(KAO_DECL_DELTA, 1, 6)
 // column-major evaluator (kao_device_t.cuh), every built schedule
 #define KAO_DECL_T(S, POP, T)                                                  \
     extern template __global__ void KAO_PERSISTENT_KERNEL_T(1, 0, S, POP, T);  \
@@ -318,8 +320,13 @@ static cudaError_t dispatch_w(kao_handle *h, const F &f, const A &a)
 }
 template <class F, class A> static cudaError_t dispatch(kao_handle *h, const F &f, const A &a)
 {
-    // one counter depth: per-lane column counts up to 255
-    return with_row_width(h->hm.W, [&](auto w) { return dispatch_w<decltype(w)::value, 5>(h, f, a); });
+    // counter depth (counter_nph): per-lane column counts up to 255, or up to 511 at 8192 padded rows
+    return with_row_width(h->hm.W, [&](auto w) -> cudaError_t {
+        constexpr int W = decltype(w)::value;
+        if (counter_nph(h->hm.Ppad) == 5) return dispatch_w<W, 5>(h, f, a);
+        if constexpr (W == 1) return dispatch_w<W, 6>(h, f, a);
+        return cudaErrorInvalidConfiguration;     // wider rows of 8192 partitions do not fit shared memory (kao_create)
+    });
 }
 // all rounds of a search in one cooperative launch, with the evaluator the session selected
 static cudaError_t launch_persistent(kao_handle *h, const PersistArgs &pa, bool delta)
@@ -512,7 +519,9 @@ static int eval_on_device(kao_handle *h, const uint32_t *d_bits, const uint8_t *
 {
     const int blocks = (n * 32 + 255) / 256;
     with_row_width(h->hm.W, [&](auto w) {
-        eval_batch_kernel<decltype(w)::value, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj);
+        constexpr int W = decltype(w)::value;
+        if (counter_nph(h->hm.Ppad) == 5) eval_batch_kernel<W, 5><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj);
+        else eval_batch_kernel<W, 6><<<blocks, 256>>>(h->prm, d_bits, d_leader, n, d_viol, d_obj);
     });
     ++h->launches;
     CUDA_TRY(cudaGetLastError());

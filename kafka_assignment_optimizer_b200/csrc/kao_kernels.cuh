@@ -728,8 +728,8 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // ------------------------------------------------------------------------------------------
 // instantiation lists.  X(W, NPH, kRack, kObj) for every evaluator configuration of a row width:
 // rack forms {general, 8-slot, 16-slot, whole-word} x objective encodings {packed entries / dense,
-// 3 mask planes} (mask planes: rows of up to 64 slots only).  One counter depth (NPH = 5: per-lane
-// column counts up to 255, i.e. every P the engine accepts).
+// 3 mask planes} (mask planes: rows of up to 64 slots only).  Counter depth NPH (counter_nph): 5 (per-lane
+// column counts up to 255, up to 7936 padded rows) for every row width, 6 for one-word rows of 8192 padded rows.
 // ------------------------------------------------------------------------------------------
 #define KAO_FOR_RACKS(X, W, NPH, O) X(W, NPH, 0, O) X(W, NPH, 3, O) X(W, NPH, 4, O) X(W, NPH, 5, O)
 #define KAO_FOR_CFGS_NARROW(X, W, NPH) KAO_FOR_RACKS(X, W, NPH, 0) KAO_FOR_RACKS(X, W, NPH, 3)

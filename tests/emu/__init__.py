@@ -42,9 +42,10 @@ class EmuSession:
             self._h = C.c_void_p()
 
     def config(self):
-        out = (C.c_int32 * 4)()
+        """Evaluator configuration of the row-major evaluator: EvalCfg<W, NPH, rack, obj> and the dense flag."""
+        out = (C.c_int32 * 5)()
         lib().kao_emu_config(self._h, out)
-        return dict(W=out[0], NPH=out[1], rack=out[2], obj=out[3])
+        return dict(W=out[0], NPH=out[1], rack=out[2], obj=out[3], dense=bool(out[4]))
 
     def set_evaluator(self, mode):
         """0: row-major evaluator; 1: column-major evaluator (csrc/kao_device_t.cuh) as the engine picks it;
@@ -85,6 +86,13 @@ class EmuSession:
         lib().kao_emu_eval(self._h, C.c_void_p(reps.ctypes.data), C.c_int32(n), C.c_void_p(v.ctypes.data),
                            C.c_void_p(o.ctypes.data))
         return v, o
+
+
+def dispatch_configs():
+    """Every (W, NPH, rack, obj) the engine's dispatch instantiates, as the emulation mirrors it."""
+    out = (C.c_int32 * 256)()
+    n = lib().kao_emu_dispatch_configs(out, C.c_int32(64))
+    return [tuple(out[4 * i:4 * i + 4]) for i in range(n)]
 
 
 def rows_charged_one_by_one():

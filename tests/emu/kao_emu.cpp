@@ -213,6 +213,20 @@ template <class Cfg> struct Run {
         }
         rebuild_lists(e);
     }
+    // the base's own evaluation as the delta kernel's full pass computes it (identity candidate, row-major
+    // evaluator): the raw violation, which a packed key would cap at its field width
+    static void base_eval(Emu &e, int &viol, int &obj)
+    {
+        const uint32_t *objT = Cfg::kObj > 0 ? e.prm.planesT : e.prm.swT;
+        emu::run_warp([&](int lane) {
+            PatchSet id;
+            id.n = 0;
+            for (int i = 0; i < kMaxOps; ++i) { id.p[i] = -1; id.ld[i] = 0xFF; }
+            int v, o;
+            eval_candidate<Cfg, true>(e.prm, e.bits.data(), e.leader.data(), objT, &e.cs, id, e.prow.data(), lane, v, o);
+            if (lane == 0) { viol = v; obj = o; }
+        });
+    }
     // delta mode (search_persistent_kernel<..., kDelta>): per-thread generator + delta evaluator on
     // the base's totals; no inverted lists here (the generator's linear-scan form)
     static unsigned long long key_delta(Emu &e, uint64_t seed, uint32_t round, uint32_t idx, uint32_t round_size,
@@ -233,7 +247,7 @@ template <class Cfg> struct Run {
 };
 
 // explicit candidate from HBM-style buffers (eval_batch_kernel): general rack form, packed entries
-template <int W> void eval_explicit(Emu &e, const uint32_t *cb, const uint8_t *cl, long long &viol, long long &obj)
+template <int W, int NPH> void eval_explicit(Emu &e, const uint32_t *cb, const uint8_t *cl, long long &viol, long long &obj)
 {
     int v = 0, o = 0;
     emu::run_warp([&](int lane) {
@@ -241,20 +255,24 @@ template <int W> void eval_explicit(Emu &e, const uint32_t *cb, const uint8_t *c
         ps.n = 0;
         for (int i = 0; i < kMaxOps; ++i) { ps.p[i] = -1; ps.ld[i] = 0xFF; }
         int lv, lo;
-        eval_candidate<EvalCfg<W, 5, 0, kObjEntries>, false>(e.prm, cb, cl, e.prm.swT, &e.cs, ps, nullptr, lane, lv, lo);
+        eval_candidate<EvalCfg<W, NPH, 0, kObjEntries>, false>(e.prm, cb, cl, e.prm.swT, &e.cs, ps, nullptr, lane, lv, lo);
         if (lane == 0) { v = lv; o = lo; }
     });
     viol = v; obj = o;
 }
 
-// kao_engine.cu: dispatch / dispatch_w / dispatch_obj
+// kao_engine.cu: dispatch / dispatch_w / dispatch_obj.  X(W, NPH, rack form, objective planes) for every
+// evaluator configuration the engine instantiates (kao_kernels.cuh: KAO_FOR_CFGS_*, kao_inst.cu)
+#define KAO_EMU_RACKS(X, W_, NPH_, O_) X(W_, NPH_, 0, O_) X(W_, NPH_, 3, O_) X(W_, NPH_, 4, O_) X(W_, NPH_, 5, O_)
+#define KAO_EMU_NARROW(X, W_, NPH_) KAO_EMU_RACKS(X, W_, NPH_, 0) KAO_EMU_RACKS(X, W_, NPH_, 3)
+#define KAO_EMU_CFGS(X) \
+    KAO_EMU_NARROW(X, 1, 5) KAO_EMU_NARROW(X, 2, 5) KAO_EMU_RACKS(X, 4, 5, 0) KAO_EMU_RACKS(X, 8, 5, 0) KAO_EMU_NARROW(X, 1, 6)
 template <class F> auto dispatch(Emu &e, F f)
 {
 #define KAO_EMU_CASE(W_, NPH_, R_, O_) \
     if (e.hm.W == W_ && e.nph == NPH_ && e.rack == R_ && e.obj == O_) return f(Run<EvalCfg<W_, NPH_, R_, O_>>{});
-#define KAO_EMU_RACKS(W_, NPH_, O_) KAO_EMU_CASE(W_, NPH_, 0, O_) KAO_EMU_CASE(W_, NPH_, 3, O_) KAO_EMU_CASE(W_, NPH_, 4, O_) KAO_EMU_CASE(W_, NPH_, 5, O_)
-#define KAO_EMU_NARROW(W_, NPH_) KAO_EMU_RACKS(W_, NPH_, 0) KAO_EMU_RACKS(W_, NPH_, 3)
-    KAO_EMU_NARROW(1, 5) KAO_EMU_NARROW(2, 5) KAO_EMU_RACKS(4, 5, 0) KAO_EMU_RACKS(8, 5, 0)
+    KAO_EMU_CFGS(KAO_EMU_CASE)
+#undef KAO_EMU_CASE
     fprintf(stderr, "kao_emu: no evaluator configuration W=%d NPH=%d rack=%d obj=%d\n", e.hm.W, e.nph, e.rack, e.obj);
     abort();
     return f(Run<EvalCfg<1, 5, 0, 0>>{});
@@ -281,7 +299,7 @@ void *kao_emu_create(const kao_problem *pb)
         plan = make_plan(m.W, m.Ppad, threads / 32, 4, m.P, m.RF, false);
     }
     if (plan.total > 227u * 1024u) { g_err = "problem too large for the shared-memory resident search kernel"; return nullptr; }
-    e->nph = 5;                                       // one counter depth (kao_engine.cu: dispatch)
+    e->nph = counter_nph(m.Ppad);                     // counter depth (kao_engine.cu: dispatch)
     e->rack = !m.hi1 ? 0 : (m.log2S == 3 ? 3 : (m.log2S == 4 ? 4 : 5));
     e->obj = (m.W <= 2 && m.nplanes == 3) ? 3 : 0;
     e->oh = m.W <= 2 && e->obj > 0;
@@ -333,11 +351,23 @@ long long kao_emu_rows_charged_one_by_one(void)
     return n;
 }
 
-// 4 ints: words per row, counter planes above the fours (NPH), rack form, objective planes
+// 5 ints: words per row, counter planes above the fours (NPH), rack form, objective planes, dense weight table
 void kao_emu_config(void *h, int32_t *out)
 {
     Emu &e = *static_cast<Emu *>(h);
-    out[0] = e.hm.W; out[1] = e.nph; out[2] = e.rack; out[3] = e.obj;
+    out[0] = e.hm.W; out[1] = e.nph; out[2] = e.rack; out[3] = e.obj; out[4] = e.prm.dense;
+}
+
+// the evaluator configurations dispatch instantiates, 4 ints each as kao_emu_config; returns their number
+int kao_emu_dispatch_configs(int32_t *out, int32_t cap)
+{
+    int n = 0;
+#define KAO_EMU_LIST(W_, NPH_, R_, O_)                                                        \
+    if (n < cap) { out[4 * n] = W_; out[4 * n + 1] = NPH_; out[4 * n + 2] = R_; out[4 * n + 3] = O_; } \
+    ++n;
+    KAO_EMU_CFGS(KAO_EMU_LIST)
+#undef KAO_EMU_LIST
+    return n;
 }
 
 void kao_emu_set_base(void *h, const int32_t *replicas)
@@ -408,12 +438,13 @@ int kao_emu_candidate_keys_delta(void *h, uint64_t seed, uint32_t round, uint32_
         }
         if (ok) ++lcnt[ld];
     }
-    int64_t bv, bo;
-    std::vector<int32_t> reps((size_t)m.P * m.RF);
-    kao_emu_get_base(h, reps.data(), &bv, &bo, nullptr);
+    // seeded with the base's raw evaluation, as the kernel's full pass of a first round: the base's packed key
+    // would hand over the field's cap instead of a saturated violation
     dispatch(e, [&](auto r) {
+        int bv, bo;
+        decltype(r)::base_eval(e, bv, bo);
         for (uint32_t i = 0; i < count; ++i)
-            keys[i] = decltype(r)::key_delta(e, seed, round, idx_begin + i, round_size, cnt.data(), lcnt.data(), rc.data(), (int)bv, (int)bo);
+            keys[i] = decltype(r)::key_delta(e, seed, round, idx_begin + i, round_size, cnt.data(), lcnt.data(), rc.data(), bv, bo);
         return 0;
     });
     return 0;
@@ -429,11 +460,13 @@ void kao_emu_eval(void *h, const int32_t *replicas, int32_t n, int64_t *violatio
         std::vector<uint8_t> cl;
         encode_replicas(m, replicas + (size_t)i * m.P * m.RF, cb, cl);
         long long v = 0, o = 0;
-        switch (m.W) {
-        case 1: eval_explicit<1>(e, cb.data(), cl.data(), v, o); break;
-        case 2: eval_explicit<2>(e, cb.data(), cl.data(), v, o); break;
-        case 4: eval_explicit<4>(e, cb.data(), cl.data(), v, o); break;
-        default: eval_explicit<8>(e, cb.data(), cl.data(), v, o); break;
+        switch (m.W) {                      // counter depth 6: only one-word rows of 8192 padded rows get past kao_emu_create
+        case 1: if (e.nph == 6) eval_explicit<1, 6>(e, cb.data(), cl.data(), v, o);
+                else eval_explicit<1, 5>(e, cb.data(), cl.data(), v, o);
+                break;
+        case 2: eval_explicit<2, 5>(e, cb.data(), cl.data(), v, o); break;
+        case 4: eval_explicit<4, 5>(e, cb.data(), cl.data(), v, o); break;
+        default: eval_explicit<8, 5>(e, cb.data(), cl.data(), v, o); break;
         }
         violation[i] = v;
         objective[i] = o;

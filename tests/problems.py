@@ -2,6 +2,10 @@
 Together they cover every layout class of the engine: W = 1/2/4/8 words per row, slot fields of
 8/16/32/64 brokers per rack, unequal racks with padding slots, removed brokers, RF raised and
 lowered, C7 lower bound > 0, and dense (tie-broken) weight tables."""
+import dataclasses
+
+import numpy as np
+
 from oracle import model as m
 
 from conftest import make_problem
@@ -37,6 +41,96 @@ SHAPES = {
     # to packed weight entries (same keys)
     "w2_rows6000": lambda: m.synthetic_problem(6000, 64, 8, 3, remove=1),
 }
+
+# Layouts and weight / bound regimes the shapes above leave out; together with them they reach every evaluator
+# configuration the engine dispatches (tests/test_layout_matrix.py checks that)
+LAYOUT_SHAPES = {
+    # whole-word rack fields with at most one replica per rack (ppr 0..1): one or two words per rack, racks of
+    # 64 slots, one 32-slot rack in a one-word row; 16-slot racks in narrow rows, 8- and 16-slot racks in wide rows
+    "rack5_w4": lambda: make_problem(120, [20, 20, 20], 2, seed=21),
+    "rack5_w8": lambda: make_problem(90, [40, 40, 40], 2, seed=22),
+    "rack5_w8_r4": lambda: make_problem(80, [33] * 4, 3, seed=23, removed=2),
+    "rack5_w1": lambda: dataclasses.replace(make_problem(60, [20], 1, seed=24), ppr_lo=0),
+    "rack5_w2": lambda: make_problem(70, [24, 24], 1, seed=25),
+    "rack4_w1": lambda: make_problem(70, [12, 12], 1, seed=26),
+    "rack4_w2": lambda: make_problem(80, [12, 12, 12], 2, seed=27),
+    "rack3_w4": lambda: make_problem(90, [6] * 12, 3, seed=28),
+    "rack3_w8": lambda: make_problem(90, [5] * 20, 3, seed=29, removed=2),
+    "rack4_w8": lambda: make_problem(90, [10] * 10, 3, seed=30),
+    # general C7 bounds (ppr 1..1) in four- and eight-word rows
+    "ppr11_w4": lambda: make_problem(100, [20, 20, 20], 3, seed=31),
+    "ppr11_w8": lambda: make_problem(100, [40, 40, 40], 3, seed=32),
+    # exactly eight term planes of the column-major evaluator, the widest cost field (key_obj_bits 24)
+    "planes8_w1": lambda: with_weight_classes(m.synthetic_problem(700, 32, 4, 3), [1000, 2000, 3000, 3500], [1, 7, 300, 595]),
+    "planes8_w2": lambda: with_weight_classes(SHAPES["cfg3_small"](), [1000, 2000, 3000, 3500], [1, 7, 300, 595]),
+    # violation fields that saturate: per-broker replica lower bounds near 65,535
+    "sat_cfg2": lambda: with_saturating_bounds(with_12bit_weights(m.synthetic_problem(256, 32, 4, 3), 50)),
+    "sat_rack5_w4": lambda: with_saturating_bounds(with_12bit_weights(LAYOUT_SHAPES["rack5_w4"](), 51)),
+}
+
+
+def with_12bit_weights(pb, seed):
+    """Packed entries with all 12 bits in use: seeded follower and leader weights in 1..4095 drawn independently
+    per current placement (a leader may weigh less than a follower), 4095 present in both."""
+    rng = np.random.RandomState(seed)
+    p, b = np.nonzero(pb.wF | pb.wL)
+    wF, wL = np.zeros(pb.wF.shape, np.int64), np.zeros(pb.wL.shape, np.int64)
+    wF[p, b], wL[p, b] = rng.randint(1, 4096, size=p.size), rng.randint(1, 4096, size=p.size)
+    wF[p[0], b[0]] = wL[p[-1], b[-1]] = 4095
+    return with_weights(pb, wF, wL)
+
+
+def with_dense_weights(pb, seed):
+    """A dense weight table: seeded weights 0..300 on every (partition, broker) cell."""
+    rng = np.random.RandomState(seed)
+    return with_weights(pb, rng.randint(0, 301, size=pb.wF.shape), rng.randint(0, 301, size=pb.wL.shape))
+
+
+def with_wide_weights(pb, seed):
+    """Seeded weights of 4096..9000 (followers) and 0..9000 (leaders) on the current placements: above the 12-bit
+    fields of packed entries, so only the dense table holds them."""
+    rng = np.random.RandomState(seed)
+    p, b = np.nonzero(pb.wF | pb.wL)
+    wF, wL = np.zeros(pb.wF.shape, np.int64), np.zeros(pb.wL.shape, np.int64)
+    wF[p, b], wL[p, b] = rng.randint(4096, 9001, size=p.size), rng.randint(0, 9001, size=p.size)
+    return with_weights(pb, wF, wL)
+
+
+def with_weight_classes(pb, follower, bonus):
+    """Partition p's i-th current replica weighs follower[(p + i) % len(follower)], its preferred replica leads
+    with bonus[p % len(bonus)] on top: len(follower) + len(bonus) term planes, each class at most once per
+    partition (RF <= len(follower))."""
+    wF, wL = np.zeros(pb.wF.shape, np.int64), np.zeros(pb.wL.shape, np.int64)
+    for p in range(pb.P):
+        for i, b in enumerate(pb.cur[p]):
+            if b >= 0:
+                wF[p, b] = follower[(p + i) % len(follower)]
+                wL[p, b] = wF[p, b] + (bonus[p % len(bonus)] if i == 0 else 0)
+    return with_weights(pb, wF, wL)
+
+
+def with_weights(pb, wF, wL):
+    return dataclasses.replace(pb, wF=wF.astype(np.uint16), wL=wL.astype(np.uint16))
+
+
+def with_saturating_bounds(pb, lo=65000):
+    """Replica lower bounds near 65,535: violations exceed the violation field of a packed key."""
+    return dataclasses.replace(pb, rep_lo=np.full(pb.B, lo, np.int32), rep_hi=np.full(pb.B, 65535, np.int32))
+
+
+# weight regimes x the layouts they are applied to: 12-bit packed entries, dense tables, weights above 12 bits,
+# weights above 12 bits in four classes (the column-major evaluator accepts them)
+_REGIMES = {
+    "w12": (with_12bit_weights, ["cfg2_rm2", "readme", "rack4_w1", "rack5_w1", "s32", "rack4_w2", "rack5_w2",
+                                 "rack5_w4", "ppr11_w8"]),
+    "dense": (with_dense_weights, ["rack4_w1", "s64_r1", "cfg3_small", "rack4_w2", "ppr11_w4", "rack3_w4", "w4_s16",
+                                   "ppr11_w8", "rack3_w8", "rack4_w8"]),
+    "wide": (with_wide_weights, ["rack5_w1", "rack5_w2", "rack5_w4", "rack5_w8"]),
+    "widecm": (lambda pb, seed: with_weight_classes(pb, [4096, 5000, 6100], [700]), ["cfg2", "cfg3_small"]),
+}
+for _regime, (_f, _bases) in _REGIMES.items():
+    for _i, _b in enumerate(_bases):
+        LAYOUT_SHAPES["%s_%s" % (_regime, _b)] = (lambda f=_f, b=_b, seed=60 + _i: f({**SHAPES, **LAYOUT_SHAPES}[b](), seed))
 
 
 def ragged_problem():
