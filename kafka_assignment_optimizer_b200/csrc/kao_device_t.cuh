@@ -45,11 +45,15 @@ namespace kao {
 //              a warp) for carry-save LOP3 (ALU pipe, 2 cycles): one hex digit per stream, 0 = a POPC per
 //              word, 1 = three per four words, 2 = two, 3 = one (Harley-Seal accumulators carried across
 //              the whole column)
+//              a third hex digit picks where the sums are formed: 0 = the popcount streams above, 1 = on the tensor
+//              cores, a binary MMA over a batch of 32 candidates (kao_device_mma.cuh; the two low digits and kSync
+//              then play no part)
 //   kThreads   threads per CTA (0 = threads_for<W>()); fewer threads = more registers per thread
 template <int W_, int kNW_ = 0, int kSync_ = 1, int kPop_ = 0x22, int kThreads_ = 0>
 struct EvalCfgT {
     static constexpr int W = W_, NPH = 5, kRack = 3, kObj = 3, kNW = kNW_;
     static constexpr int kSync = kSync_, kPop = kPop_, kThreads = kThreads_;
+    static constexpr int kSums = kPop_ >> 8;
     static constexpr bool kTrans = true;
 };
 constexpr int kTPlanes = 2;
@@ -405,9 +409,10 @@ __device__ __forceinline__ uint32_t a_gather(int b, int w, const uint32_t *bitsT
     return out;
 }
 // Row p of the base becomes (newrow, newld): every lane rewrites bit p of its own slots' words in both
-// transposed planes, lanes 0..7 bit p of one term plane each, the next 4 W lanes bit p of one rack-field plane each
+// transposed planes, lanes 0..7 bit p of one term plane each, the next 4 W lanes bit p of one rack-field plane each,
+// with kS the next four bit p of one shortfall plane each (kao_device_mma.cuh)
 // (the whole warp calls this; the row-major base itself is patched by the caller).
-template <int W>
+template <int W, bool kS = false>
 __device__ __forceinline__ void t_patch_row(const Params &d, uint32_t *T, uint32_t *Z, int nW, int p, const uint32_t (&newrow)[W],
                                             uint32_t newld, int lane)
 {
@@ -433,6 +438,10 @@ __device__ __forceinline__ void t_patch_row(const Params &d, uint32_t *T, uint32
         const int b = lane - kZPlanes;
         uint32_t &word = Z[lane * nW + w];
         word = ((newrow[b >> 2] >> (8 * (b & 3))) & 0xFFu) ? (word | bit) : (word & ~bit);
+    } else if (kS && lane < kZPlanes + kAPlanes<W>() + 4) {
+        const int k = lane - kZPlanes - kAPlanes<W>(), short_by = max(d.RF - row_count<W>(newrow), 0);
+        uint32_t &word = Z[lane * nW + w];
+        word = ((short_by >> k) & 1) ? (word | bit) : (word & ~bit);
     }
 }
 

@@ -274,7 +274,7 @@ template <bool kDelta> struct LaunchPersistent {
         if (e != cudaSuccess) return e;
         Params prm = h->prm;
         // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch)
-        SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF)
+        SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF, cfg_mma<Cfg>())
                         : (kDelta && Cfg::W > 2) ? make_plan_delta_wide(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF) : h->plan;
         if (plan.total > 227u * 1024u) return cudaErrorInvalidConfiguration;
         uint64_t seed = a.seed; uint32_t fr = a.first_round, rounds = a.rounds, rs = a.round_size;

@@ -7,6 +7,7 @@
 #pragma once
 #include "kao_device.cuh"
 #include "kao_device_t.cuh"
+#include "kao_device_mma.cuh"
 #include "kao_plan.hpp"
 
 #include <cstdint>
@@ -26,6 +27,12 @@ template <class Cfg> constexpr int cfg_threads()
 {
     if constexpr (Cfg::kTrans) return Cfg::kThreads ? Cfg::kThreads : threads_for<Cfg::W>();
     else return threads_for<Cfg::W>();
+}
+// does a configuration form its sums on the tensor cores (column-major, kao_device_mma.cuh)
+template <class Cfg> __host__ __device__ constexpr bool cfg_mma()
+{
+    if constexpr (Cfg::kTrans) return Cfg::kSums == 1;
+    else return false;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -74,8 +81,8 @@ __device__ __forceinline__ void build_oh_plane(uint32_t *s_bits, const uint8_t *
 
 // Column-major evaluator (kao_device_t.cuh): the two transposed planes and the term planes of the objective
 // are gathered once per launch from the staged row-major base (2 * W words per partition at off_sw, the term
-// planes at off_z).
-template <int W, int THREADS>
+// planes at off_z; kS: and the shortfall planes of the tensor-core form behind the rack-field planes).
+template <int W, int THREADS, bool kS = false>
 __device__ __forceinline__ void build_t_planes(const Params &d, uint32_t *T, uint32_t *Z, const uint32_t *s_bits, const uint8_t *s_leader)
 {
     constexpr int NSL = 32 * W;
@@ -86,6 +93,8 @@ __device__ __forceinline__ void build_t_planes(const Params &d, uint32_t *T, uin
     }
     for (int o = threadIdx.x; o < kZPlanes * nW; o += THREADS) Z[o] = z_gather<W>(d, o / nW, o % nW, s_bits, s_leader);
     for (int o = threadIdx.x; o < kAPlanes<W>() * nW; o += THREADS) Z[kZPlanes * nW + o] = a_gather<W>(o / nW, o % nW, s_bits, d.Ppad);
+    if constexpr (kS)
+        for (int o = threadIdx.x; o < kSPlanes * nW; o += THREADS) Z[(kZPlanes + kAPlanes<W>()) * nW + o] = s_gather<W>(d, o / nW, o % nW, s_bits);
     __syncthreads();
 }
 
@@ -422,7 +431,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
     }
     mbar_wait(s_bar, 0);
     if constexpr (has_oh_plane<Cfg>()) build_oh_plane<W, THREADS>(s_bits, s_leader, d.Ppad);
-    if constexpr (Cfg::kTrans) build_t_planes<W, THREADS>(d, s_sw, s_z, s_bits, s_leader);
+    if constexpr (Cfg::kTrans) build_t_planes<W, THREADS, cfg_mma<Cfg>()>(d, s_sw, s_z, s_bits, s_leader);
     rebuild_lists<THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
     if constexpr (Cfg::kTrans) {
         // s_counts[2] = partitions whose leader slot is not one of their replicas (0 for every base the engine builds or
@@ -495,6 +504,52 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                 best = w < best ? w : best;
             }
             if (all_keys) return;                                   // key dump only: the base stays as it is
+        } else if constexpr (cfg_mma<Cfg>()) {
+            // ---- column-major evaluator, sums on the tensor cores (kao_device_mma.cuh): candidates are generated 32 at a
+            // time, one per LANE, as below, then the warp evaluates all 32 together; lane (g, t) ends with the
+            // violation and objective of candidate mma_lane_candidate(lane) of the batch
+            Gen<W, true, true> tg;        // compact code (row_kth keeps its loop), same candidates
+            tg.bitsT = s_bits; tg.leader = s_leader; tg.cs = s_cs; tg.d = &d; tg.prow = nullptr; tg.lane = 0;
+            tg.D = s_D; tg.DL = s_DL; tg.nD = s_counts[0]; tg.nL = s_counts[1];
+            tg.T = s_sw; tg.tnW = t_words(d.Ppad); tg.t_leaders_valid = s_counts[2] == 0;    // "first holder of slot s": plane scan
+            uint32_t *batch = s_prow + (size_t)warp * 32 * batch_stride<W>();
+            const uint32_t j = (uint32_t)mma_lane_candidate(lane);
+            for (uint32_t it0 = 0; it0 < iters; it0 += 32) {
+                mma_clear_batch<W>(batch, lane);
+                __syncwarp();
+                {
+                    const uint32_t idx = first + warp + (it0 + lane) * stride;
+                    PatchSet ps;
+                    uint32_t rows[kMaxOps][W];
+                    ps.n = 0;
+#pragma unroll
+                    for (int i = 0; i < kMaxOps; ++i) {
+                        ps.p[i] = -1; ps.ld[i] = 0xFF;
+#pragma unroll
+                        for (int w = 0; w < W; ++w) rows[i][w] = 0;
+                    }
+                    if (it0 + lane < iters && idx < pp.idx_hi) tg.run(seed, round, idx, round_size, ps, rows);
+                    int pviol, pobj, pcount;
+                    patch_terms<W>(d, ps, rows, pviol, pobj, pcount);
+                    mma_park_patch<W>(ps, rows, pviol, pobj, batch, lane);
+                }
+                __syncwarp();
+                int viol, obj;
+                eval_batch_mma<Cfg>(d, s_cs, s_sw, t_words(d.Ppad), s_z, batch, lane, viol, obj);
+                const uint32_t idx = first + warp + (it0 + j) * stride;
+                if (it0 + j < iters && idx < pp.idx_hi) {
+                    const unsigned long long key = pack_key(viol, obj, idx, d.key_obj_bits);
+                    if (all_keys) all_keys[idx - pp.idx_lo] = key;
+                    best = key < best ? key : best;                 // equal (violation, cost): the lowest index
+                }
+                __syncwarp();                                               // the batch is consumed before it is refilled
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, best, o);
+                best = w < best ? w : best;
+            }
+            if (all_keys) return;                                           // key dump only: the base stays as it is
         } else if constexpr (Cfg::kTrans) {
             // ---- column-major evaluator: candidates are generated 32 at a time, one per LANE (per-thread
             // generator over the round's inverted lists), then evaluated in full one after the other by the warp
@@ -689,7 +744,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                             uint32_t newrow[W];
 #pragma unroll
                             for (int w = 0; w < W; ++w) newrow[w] = gen.prow[i * W + w];
-                            t_patch_row<W>(d, s_sw, s_z, t_words(d.Ppad), ps.p[i], newrow, ps.ld[i], lane);
+                            t_patch_row<W, cfg_mma<Cfg>()>(d, s_sw, s_z, t_words(d.Ppad), ps.p[i], newrow, ps.ld[i], lane);
                         }
                     }
                 }
@@ -742,10 +797,10 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // Column-major kernels: X(sync, pop, threads) for every built schedule (kao_set_schedule); each is
 // instantiated for W = 1, 2 and for 32 partition words (compile-time offsets) / any word count.
 #define KAO_FOR_SCHEDULES(X) \
-    X(4, 0x22, 1024) X(1, 0x22, 896) X(4, 0x22, 896) X(4, 0x22, 768) X(4, 0x12, 896) X(2, 0x22, 896)
-#define KAO_SCHEDULE_DEFAULT_SYNC 4
-#define KAO_SCHEDULE_DEFAULT_POP 0x22
-#define KAO_SCHEDULE_DEFAULT_THREADS 1024
+    X(1, 0x100, 512) X(4, 0x22, 1024) X(1, 0x22, 896) X(4, 0x22, 896) X(4, 0x12, 896) X(2, 0x22, 896)
+#define KAO_SCHEDULE_DEFAULT_SYNC 1
+#define KAO_SCHEDULE_DEFAULT_POP 0x100
+#define KAO_SCHEDULE_DEFAULT_THREADS 512
 #define KAO_PERSISTENT_KERNEL_T(W, NW, S, POP, T)                                                            \
     search_persistent_kernel<EvalCfgT<W, NW, S, POP, T>, T, false>(Params, SmemPlan, uint64_t, uint32_t, uint32_t, \
                                                                     uint32_t, unsigned long long *, unsigned int *, P2P, \

@@ -28,8 +28,9 @@ static_assert(batch_stride_words(1) % 8 == 4 && batch_stride_words(2) % 8 == 4, 
 
 // prow_words_per_warp: per-warp scratch for patched rows (kMaxOps * W), or a whole batch of candidates
 // lists: 1 stage the inverted lists of the per-thread generator if they fit, 0 never, -1 = for rows of up to 64 slots
+// round_tables: the per-round tables of the delta kernels (at off_totals; the MMA column-major plan has none)
 inline SmemPlan make_plan(int W, int Ppad, int warps, int obj_words_per_row, int P, int RF, bool oh_plane,
-                          int prow_words_per_warp = 0, int lists = -1, int z_bytes = 0)
+                          int prow_words_per_warp = 0, int lists = -1, int z_bytes = 0, bool round_tables = true)
 {
     if (prow_words_per_warp <= 0) prow_words_per_warp = kMaxOps * W;
     SmemPlan s;
@@ -46,7 +47,7 @@ inline SmemPlan make_plan(int W, int Ppad, int warps, int obj_words_per_row, int
     s.off_red = o;    o += (uint32_t)(warps + 4) * 8;      // + early-stop state behind the per-warp minima
     s.off_bar = o;    o += 16;
     s.off_lists = o;  o += (uint32_t)Ppad * 4 + 16 + 2 * 36 * 4;   // D, DL (u16 each), counts, scan scratch
-    s.off_totals = o; o += (256 + 256 + 32 + 4 + 256 + 2 * 258 + 4) * 4;  // per-round tables (kao_kernels.cuh, RoundTables): cnt,
+    s.off_totals = o; o += round_tables ? (256 + 256 + 32 + 4 + 256 + 2 * 258 + 4) * 4 : 0;  // per-round tables (kao_kernels.cuh, RoundTables): cnt,
                                                                            // lcnt, rc, base (viol, obj), led counts, list offsets, flag
     s.off_inv = o;
     s.cap_hold = s.cap_led = 0;
@@ -64,15 +65,18 @@ inline SmemPlan make_plan(int W, int Ppad, int warps, int obj_words_per_row, int
 }
 
 // shared-memory plan of a column-major kernel: the two transposed planes + the term planes in place of the
-// objective table, a batch of candidates per warp (the per-thread generator scans the transposed planes: no inverted lists)
-inline SmemPlan make_plan_t(int W, int Ppad, int threads, int P, int RF)
+// objective table, a batch of candidates per warp (the per-thread generator scans the transposed planes: no inverted lists).
+// mma: the tensor-core form (kao_device_mma.cuh) keeps four shortfall planes behind the rack-field planes
+// (16 nW bytes, at most 4 KB) and has no per-round tables (5,296 bytes): it fits wherever the other form does.
+inline SmemPlan make_plan_t(int W, int Ppad, int threads, int P, int RF, bool mma = false)
 {
     // make_plan sizes the area at off_sw in words per partition of Ppad: the transposed planes hold t_words(Ppad)
     // words per slot, which is Ppad / 32 or (more than 1024 partitions) up to 31 words more — one extra word per
     // partition covers that for every Ppad the evaluator accepts
     const int nW = t_words(Ppad);
     const int per_row = (kTPlanes * W * 32 * nW + Ppad - 1) / Ppad;
-    return make_plan(W, Ppad, threads / 32, per_row, P, RF, false, 32 * batch_stride_words(W), 0, (kZPlanes + 4 * W) * nW * 4);      // term planes + rack-field planes
+    return make_plan(W, Ppad, threads / 32, per_row, P, RF, false, 32 * batch_stride_words(W), 0,
+                     (kZPlanes + 4 * W + (mma ? 4 : 0)) * nW * 4, !mma);        // term planes + rack-field planes (+ shortfall planes)
 }
 // does the column-major evaluator cover this layout (kao_create; tests/emu asks the same question)
 inline bool column_major_fits(int W, int Ppad, int threads, int P, int RF)
