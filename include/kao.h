@@ -96,6 +96,9 @@ typedef struct kao_options {
                                          single-GPU search (nothing is exchanged between the GPUs), instead of sharding every
                                          round of every restart; same result as one GPU.  The way to use several GPUs for
                                          the recipe that finds optima: many short independent searches (INTEGRATION.md 5) */
+#define KAO_FLAG_LP_BOUND 0x1000u     /* feasible result: kao_result.objective_bound becomes the minimum of the bound above and the
+                                         Lagrangian LP bound of kao_lp_bound (GPU, at most KAO_LP_ITERATIONS iterations, aimed at
+                                         the returned objective) -- the certificate that proves optima the flow bound cannot */
 #define KAO_FLAG_PATIENCE(n) ((uint32_t)(n) << 16)  /* stop a search after n (<= 65535) rounds without a better key */
 
 typedef struct kao_result {
@@ -113,7 +116,8 @@ typedef struct kao_result {
     double total_ms;          /* wall time of the call incl. host<->device copies */
     int64_t objective_bound;  /* an upper bound on the objective of ANY feasible assignment: per partition the best
                                  leader + best RF-1 followers (C3..C7 ignored), or with KAO_FLAG_BOUND the much
-                                 tighter flow bound of kao_objective_bound; lp_solve's optimum (README.md:135-136)
+                                 tighter flow bound of kao_objective_bound, and with KAO_FLAG_LP_BOUND at most the
+                                 Lagrangian LP bound of kao_lp_bound; lp_solve's optimum (README.md:135-136)
                                  lies between `objective` and this */
     int32_t optimal;          /* 1: feasible and objective == objective_bound, i.e. PROVEN optimal; 0: not proven
                                  (the search is a heuristic: it never claims more than the bound shows) */
@@ -136,6 +140,22 @@ int kao_solve(const kao_problem *pb, const kao_options *opt, kao_result *res);
  * (placement under C1/C3/C6/C7, leadership under C2/C4; only their coupling is dropped), found by cancelling
  * negative cycles from that assignment; never above the first bound.  objective == bound proves optimality. */
 int kao_objective_bound(const kao_problem *pb, const int32_t *replicas, int64_t *bound);
+
+/* The Lagrangian LP bound (docs/MODEL.md §9): C3, C4 and C6 dualised with multipliers u of KAO_LP_FRACTION_BITS
+ * fractional bits; for ANY u, L(u) = sum over those rows of (u > 0 ? u*hi : u*lo) + sum over partitions of the best row
+ * under the reduced weights bounds the objective of every feasible assignment from above, and its minimum is the value of
+ * the LP relaxation of the whole 0/1 program.  A subgradient iteration in exact integer arithmetic (one cooperative GPU
+ * launch) aims at the objective T of `replicas`, a FEASIBLE assignment ([P*RF], leader first), and stops when the bound
+ * reaches T (objective == bound proves optimality), when the subgradient or the step vanishes, or after max_iterations
+ * (1 .. KAO_MAX_LP_ITERATIONS).  bound = floor(min over the iterations of L / 2^KAO_LP_FRACTION_BITS); iterations_run =
+ * evaluations of L; multipliers (optional, [2B + R]: C3 per broker, C4 per broker, C6 per rack) = the u of that
+ * minimum.  The result is the same on every GPU and in every run.  KAO_E_ARG for an infeasible or malformed
+ * assignment, KAO_E_CUDA without a device (there is no CPU path). */
+#define KAO_LP_FRACTION_BITS 20
+#define KAO_LP_ITERATIONS 4096              /* the cap kao_solve uses with KAO_FLAG_LP_BOUND */
+#define KAO_MAX_LP_ITERATIONS (1u << 20)
+int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int32_t device, uint32_t max_iterations,
+                 int64_t *bound, uint32_t *iterations_run, int64_t *multipliers);
 
 /* Evaluate n explicit assignments (each [P*RF] replica lists, leader first, -1 padded) on the
  * GPU with the same evaluator the search uses: C1..C7 violation amount and objective. */

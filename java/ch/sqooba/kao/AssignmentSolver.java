@@ -15,7 +15,7 @@ import java.util.*;
  * <pre>
  * java -Djava.library.path=. ch.sqooba.kao.AssignmentSolver --assignment current.json \
  *      --brokers 0,1,2,...,18 --racks 0:a,1:b,... [--rf 2] [--rounds 256] [--round-size 32768]
- *      [--restarts 1] [--seed 24301] [--device 0] [--gpus 1] [--spread-restarts] [--delta] [--patience N] [--certificate] [--stats]
+ *      [--restarts 1] [--seed 24301] [--device 0] [--gpus 1] [--spread-restarts] [--delta] [--patience N] [--certificate] [--lp-certificate] [--stats]
  * </pre>
  * in:  the JSON `kafka-reassign-partitions --generate` prints (README.md:52-63), the target broker list
  *      (README.md:48), broker:rack pairs (README.md:27-29);
@@ -137,20 +137,21 @@ public final class AssignmentSolver {
     private static int usage() {
         System.err.println("usage: AssignmentSolver --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
                 + "       [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--gpus 1]"
-                + " [--spread-restarts] [--delta] [--patience N] [--certificate] [--stats]");
+                + " [--spread-restarts] [--delta] [--patience N] [--certificate] [--lp-certificate] [--stats]");
         return 2;
     }
 
     /** Exit status as kao-cli: 0 ok, 1 error, 2 usage, 3 no assignment satisfying every constraint was found. */
     public static void main(String[] argv) throws IOException {
         Map<String, String> a = new HashMap<>();
-        boolean stats = false, delta = false, spread = false, certificate = false;
+        boolean stats = false, delta = false, spread = false, certificate = false, lpCertificate = false;
         for (int i = 0; i < argv.length; i++) {
             String k = argv[i];
             if (k.equals("--stats")) { stats = true; continue; }
             if (k.equals("--delta")) { delta = true; continue; }
             if (k.equals("--spread-restarts")) { spread = true; continue; }
             if (k.equals("--certificate")) { certificate = true; continue; }
+            if (k.equals("--lp-certificate")) { lpCertificate = true; continue; }   // Lagrangian LP bound on the GPU
             if (!k.startsWith("--") || i + 1 >= argv.length) System.exit(usage());
             a.put(k.substring(2), argv[++i]);
         }
@@ -174,6 +175,7 @@ public final class AssignmentSolver {
             if (delta) flags |= FLAG_DELTA;
             if (spread) flags |= FLAG_SPREAD_RESTARTS;
             if (certificate) flags |= FLAG_BOUND;
+            if (lpCertificate) flags |= KaoNative.FLAG_LP_BOUND;
             if (a.containsKey("patience")) flags |= Math.min(65535, Math.max(0, Integer.parseInt(a.get("patience")))) << 16;
             long[] st = new long[8];
             int[][] res = solve(current, brokers, racks, rf, Long.decode(a.getOrDefault("seed", "24301")),

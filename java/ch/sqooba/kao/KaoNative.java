@@ -9,6 +9,11 @@ public final class KaoNative {
 
     private KaoNative() {}
 
+    /** kao_options.flags: kao_result objective bound from the flow relaxations (host) */
+    public static final int FLAG_BOUND = 0x400;
+    /** kao_options.flags: also the Lagrangian LP bound on the GPU (docs/MODEL.md 9): proves optima the flow bound cannot */
+    public static final int FLAG_LP_BOUND = 0x1000;
+
     /** kao_version() */
     public static native int version();
 
@@ -24,7 +29,7 @@ public final class KaoNative {
      * @param cur     [P*RFcur] current assignment, leader first, -1 = absent (README.md:52-63)
      * @param replicasOut [P*RF] result, leader first (README.md:67-78, :88)
      * @param nGpus   1, or N: every round is sharded over N GPUs of this process (device .. device+N-1)
-     * @param flags   kao_options.flags: restarts | KAO_FLAG_DELTA (0x100) | KAO_FLAG_SPREAD_RESTARTS (0x800) | KAO_FLAG_PATIENCE(n) (n << 16)
+     * @param flags   kao_options.flags: restarts | KAO_FLAG_DELTA (0x100) | KAO_FLAG_SPREAD_RESTARTS (0x800) | FLAG_BOUND | FLAG_LP_BOUND | KAO_FLAG_PATIENCE(n) (n << 16)
      * @param statsOut [8] objective, violation, replica moves, candidates evaluated, objective upper
      *                bound, proven optimal (0/1), rounds run, GPUs used
      * @return 0 ok, 1 no feasible assignment found; throws KaoException on argument/CUDA errors

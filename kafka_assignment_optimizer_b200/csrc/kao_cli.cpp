@@ -258,7 +258,7 @@ int usage()
 {
     std::fprintf(stderr,
                  "usage: kao-cli --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
-                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--emit-lp] [--stats]\n");
+                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--emit-lp] [--stats]\n");
     return 2;
 }
 
@@ -267,7 +267,7 @@ int usage()
 int main(int argc, char **argv)
 {
     std::map<std::string, std::string> a;
-    bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false;
+    bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false, lp_certificate = false;
     for (int i = 1; i < argc; ++i) {
         std::string k = argv[i];
         if (k == "--emit-lp") { emit = true; continue; }
@@ -276,6 +276,7 @@ int main(int argc, char **argv)
         if (k == "--row-major") { rowmajor = true; continue; }
         if (k == "--spread-restarts") { spread = true; continue; }   // --gpus N: the restarts side by side, one per GPU at a time
         if (k == "--certificate") { certificate = true; continue; }  // flow bound: --stats can then say "proven optimal"
+        if (k == "--lp-certificate") { lp_certificate = true; continue; }  // Lagrangian LP bound (GPU): proves what the flow bound cannot
         if (k == "--column-major") continue;                  // accepted for old scripts: it is the default now
         if (k.rfind("--", 0) != 0 || i + 1 >= argc) return usage();
         a[k.substr(2)] = argv[++i];
@@ -325,6 +326,7 @@ int main(int argc, char **argv)
         if (rowmajor) opt.flags |= KAO_FLAG_ROW_MAJOR;        // measurements: the other full evaluator, same result
         if (spread) opt.flags |= KAO_FLAG_SPREAD_RESTARTS;
         if (certificate) opt.flags |= KAO_FLAG_BOUND;
+        if (lp_certificate) opt.flags |= KAO_FLAG_LP_BOUND;
         if (a.count("patience")) opt.flags |= KAO_FLAG_PATIENCE(std::min(65535, std::max(0, std::atoi(a["patience"].c_str()))));
         std::vector<int32_t> reps((size_t)m.P * m.RF, -1);
         kao_result res{};

@@ -6,6 +6,7 @@
 #include "kao_kernels.cuh"
 #include "kao_host.hpp"
 #include "kao_bound.hpp"
+#include "kao_lagrange.hpp"
 #include "../../include/kao.h"
 
 #include <chrono>
@@ -1119,6 +1120,16 @@ static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result 
     res->objective_bound = objective_upper_bound(s.hm, *pb);
     if ((opt->flags & KAO_FLAG_BOUND) && res->feasible)
         res->objective_bound = objective_flow_bound(s.hm, *pb, res->replicas, res->objective_bound);
+    if ((opt->flags & KAO_FLAG_LP_BOUND) && res->feasible) {
+        // the Lagrangian LP bound aimed at the returned objective (MODEL §9), on the first GPU of the call
+        int64_t lp = 0;
+        uint32_t its = 0;
+        std::string why;
+        rc = lagrange_bound_device(*pb, devs[0], res->objective, KAO_LP_ITERATIONS, wait_budget_ns(), &lp, &its, nullptr, nullptr, why);
+        if (rc != KAO_OK) return fail(rc, why);
+        res->objective_bound = std::min(res->objective_bound, lp);
+        stamp(t0, "LP bound computed");
+    }
     res->optimal = res->feasible && res->objective == res->objective_bound;
     res->key_obj_bits = s.hm.key_obj_bits;
     res->n_gpus = world;
@@ -1154,6 +1165,25 @@ extern "C" int kao_objective_bound(const kao_problem *pb, const int32_t *replica
         *bound = objective_upper_bound(m, *pb);
         if (replicas) *bound = objective_flow_bound(m, *pb, replicas, *bound);
         return KAO_OK;
+    });
+}
+extern "C" int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int32_t device, uint32_t max_iterations,
+                            int64_t *bound, uint32_t *iterations_run, int64_t *multipliers)
+{
+    return guarded([&] {
+        if (!pb || !replicas || !bound || !iterations_run) return fail(KAO_E_ARG, "null argument");
+        if (max_iterations < 1 || max_iterations > KAO_MAX_LP_ITERATIONS)
+            return fail(KAO_E_ARG, "max_iterations must be 1..KAO_MAX_LP_ITERATIONS (2^20)");
+        HostModel m;
+        std::string why;
+        if (!build_host_model(*pb, m, why)) return fail(KAO_E_ARG, why);
+        int64_t T = 0;
+        if (!feasible_objective(*pb, replicas, T, why)) return fail(KAO_E_ARG, why);
+        int ndev = 0;
+        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(KAO_E_CUDA, "no CUDA device: libkao has no CPU path");
+        if (device < 0 || device >= ndev) return fail(KAO_E_ARG, "bad device ordinal");
+        const int rc = lagrange_bound_device(*pb, device, T, max_iterations, wait_budget_ns(), bound, iterations_run, multipliers, nullptr, why);
+        return rc == KAO_OK ? KAO_OK : fail(rc, why);
     });
 }
 extern "C" int kao_create(const kao_problem *pb, int32_t device, kao_handle **out) { return guarded([&] { return create_handle(pb, device, out); }); }

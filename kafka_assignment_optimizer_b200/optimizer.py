@@ -98,6 +98,25 @@ def objective_bound(pb: Problem, replicas=None) -> int:
     return out.value
 
 
+LP_ITERATIONS = 4096          # KAO_LP_ITERATIONS: the cap kao_solve uses with lp_bound=True
+LP_FRACTION_BITS = 20         # KAO_LP_FRACTION_BITS of the multipliers
+
+
+def lp_bound(pb: Problem, replicas, device: int = 0, max_iterations: int = LP_ITERATIONS, multipliers: bool = False):
+    """The Lagrangian LP bound of kao_lp_bound (docs/MODEL.md 9; GPU): an upper bound on the objective of every
+    feasible assignment, aimed at the objective of `replicas` (a feasible assignment [P, RF], leader first).  -> (bound,
+    iterations run), or (bound, iterations run, multipliers int64[2B + R] with LP_FRACTION_BITS fractional bits)."""
+    r = np.ascontiguousarray(replicas, dtype=np.int32)
+    if r.shape != (pb.P, pb.RF):
+        raise ValueError("replicas must be [P, RF]")
+    out, its = C.c_int64(), C.c_uint32()
+    u = np.zeros(2 * pb.B + pb.R, np.int64)
+    _check(load_library().kao_lp_bound(_CProblem(pb).ref(), C.c_void_p(r.ctypes.data), C.c_int32(device),
+                                       C.c_uint32(max_iterations), C.byref(out), C.byref(its),
+                                       C.c_void_p(u.ctypes.data)))
+    return (out.value, its.value, u) if multipliers else (out.value, its.value)
+
+
 class _CProblem:
     """Keeps contiguous numpy buffers alive next to the C struct that points into them."""
 
@@ -295,15 +314,16 @@ class Session:
 def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 1 << 15,
           device: int = 0, require_feasible: bool = False, restarts: int = 1, delta: bool = False,
           patience: int = 0, row_major: bool = False, n_gpus: int = 1, device_mask: int = 0,
-          tight_bound: bool = False, spread_restarts: bool = False) -> SolveResult:
+          tight_bound: bool = False, spread_restarts: bool = False, lp_bound: bool = False) -> SolveResult:
     """One blocking kao_solve from host buffers (tables up, winner down).  n_gpus > 1: every round is sharded
     over that many GPUs of this process (devices device .. device+n_gpus-1, or those of device_mask), or with
     spread_restarts the restarts run side by side, one single-GPU search per GPU at a time; either way the
-    result is the same as on one GPU with the same arguments."""
+    result is the same as on one GPU with the same arguments.  tight_bound / lp_bound: objective_bound from the flow
+    bound (KAO_FLAG_BOUND) / also from the Lagrangian LP bound (KAO_FLAG_LP_BOUND); either can prove optimality."""
     lib = load_library()
     cp = _CProblem(pb)
     reps = np.full((pb.P, pb.RF), -1, np.int32)
-    flags = (max(1, min(255, restarts)) | (0x100 if delta else 0) | (0x200 if row_major else 0) | (0x400 if tight_bound else 0) | (0x800 if spread_restarts else 0) |
+    flags = (max(1, min(255, restarts)) | (0x100 if delta else 0) | (0x200 if row_major else 0) | (0x400 if tight_bound else 0) | (0x800 if spread_restarts else 0) | (0x1000 if lp_bound else 0) |
              (max(0, min(65535, patience)) << 16))
     opt = _KaoOptions(seed & (2 ** 64 - 1), rounds, round_size, device, flags, n_gpus, device_mask)
     res = _KaoResult()
@@ -335,7 +355,8 @@ class AssignmentOptimizer:
     printed plus the target broker list and topology, get the reassignment JSON back."""
 
     def __init__(self, seed: int = 0x5EED, rounds: int = 256, round_size: int = 1 << 15, device: int = 0, **solve_options):
-        """solve_options: anything else `solve` takes (restarts, patience, delta, n_gpus, spread_restarts, tight_bound)."""
+        """solve_options: anything else `solve` takes (restarts, patience, delta, n_gpus, spread_restarts, tight_bound,
+        lp_bound)."""
         self.seed, self.rounds, self.round_size, self.device = seed, rounds, round_size, device
         self.solve_options = solve_options
 
