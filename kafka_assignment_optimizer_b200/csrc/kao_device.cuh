@@ -192,7 +192,10 @@ struct PatchSet {
 // kThread = false: one warp generates one candidate cooperatively (patched rows go to `prow`);
 // kThread = true : every thread generates its own candidate (patched rows go to the caller's registers).
 // kSmall: compact code (row_kth), same candidates.
-template <int W, bool kThread = false, bool kSmall = false> struct Gen {
+// kMerged (thread mode with transposed planes): the four link kinds of a later operation share one partition search,
+// one row read, one REPLACE and one LEADER step, so that a warp whose lanes take different links runs each of those
+// once instead of once per link kind.  Same candidates.
+template <int W, bool kThread = false, bool kSmall = false, bool kMerged = false> struct Gen {
     const uint32_t *bitsT;   // base (shared or global)
     const uint8_t *leader;
     const Consts *cs;
@@ -362,6 +365,37 @@ template <int W, bool kThread = false, bool kSmall = false> struct Gen {
         }
         return -1;
     }
+    // find_from with the kind chosen at run time: one scan of the transposed planes whatever the kind (kMerged)
+    __device__ __forceinline__ int find_from_any(const PatchSet &ps, int p0, int src, int kind) const
+    {
+        if (src < 0 || src >= W * 32) return -1;
+        if (T != nullptr && (kind != 1 || t_leaders_valid)) {
+            constexpr int NSL = 32 * W;
+            const int nWq = (d->P + 31) >> 5;
+            const uint32_t *r0 = T + (size_t)src * tnW, *r1 = T + (size_t)(NSL + src) * tnW;
+            const int sw = t_swizzled(tnW) ? 4 * (src & 7) : 0;
+            // kind 0: r0; 1: r1; 2: r0 & ~r1
+            const uint32_t *ra = kind == 1 ? r1 : r0;
+            const bool minus_led = kind == 2;
+            int w = p0 >> 5;
+            uint32_t keep = ~0u << (p0 & 31);
+            for (int i = 0; i <= nWq; ++i) {
+                const int pw = w ^ sw;
+                uint32_t m = ra[pw];
+                if (minus_led) m &= ~r1[pw];
+                m &= keep;
+                if (i == nWq) m &= ~(~0u << (p0 & 31));
+#pragma unroll
+                for (int j = 0; j < kMaxOps; ++j)
+                    if ((ps.p[j] >> 5) == w) m &= ~(1u << (ps.p[j] & 31));
+                if (m) return 32 * w + __ffs(m) - 1;
+                keep = ~0u;
+                w = (w + 1 == nWq) ? 0 : w + 1;
+            }
+            return -1;
+        }
+        return kind == 0 ? find_from<0>(ps, p0, src) : (kind == 1 ? find_from<1>(ps, p0, src) : find_from<2>(ps, p0, src));
+    }
 
     // docs/MODEL.md §5 — must stay bit-identical to the restated generator the tests check against
     __device__ void run(uint64_t seed, uint32_t round, uint32_t idx, uint32_t round_size, PatchSet &ps,
@@ -429,6 +463,70 @@ template <int W, bool kThread = false, bool kSmall = false> struct Gen {
         }
         if (nops == 1) return;
         philox4x32_10(idx, round, 1u, kTag, (uint32_t)seed, (uint32_t)(seed >> 32), s);
+        if constexpr (kMerged) {
+            for (int k = 1; k < nops; ++k) {
+                const uint32_t link = (ctl >> (4 + 3 * (k - 1))) & 3u;
+                const bool close = (ctl >> (6 + 3 * (k - 1))) & 1u;
+                const uint32_t ra = (k == 1) ? s[0] : s[2], rb = (k == 1) ? s[1] : s[3];
+                const int start = (int)mulhi32(ra, (uint32_t)P);
+                int olo = (lo >= 0 && lo < 256) ? (int)cs->order_of_slot[lo] : 0xFF;
+                if (olo >= B) olo = 0;
+                uint32_t rq[W], lq;
+                const bool match = cycle && ((ctl >> (11 + 2 * (k - 1))) & 1u);
+                // the partition: R-pull takes `start` itself, the others search from it — R-push for a holder of hi
+                // (of its leader / a follower on hi when the roles match), L-push for the leader on hi, L-pull for a
+                // follower on lo
+                int q = start;
+                if (link == 1) {
+                    bool t = false;
+#pragma unroll
+                    for (int i = 0; i < kMaxOps; ++i) t |= (ps.p[i] == q);
+                    if (t) return;
+                } else {
+                    const int kind = link == 0 ? (!match ? 0 : (moved_leader ? 1 : 2)) : (link == 2 ? 1 : 2);
+                    q = find_from_any(ps, start, link == 3 ? lo : hi, kind);
+                    if (q < 0) return;
+                }
+                read_row(q, rq, lq);
+                if (link <= 1) {                               // R-push / R-pull: one REPLACE
+                    int a, o;
+                    if (link == 0) {
+                        if (!row_has<W>(rq, hi)) return;       // led from hi without a replica there (malformed base)
+                        a = hi;
+                        o = close ? olo : (int)mulhi32(rb, (uint32_t)B);
+                    } else {
+                        const int nq = row_count<W>(rq);
+                        if (nq == 0) return;
+                        a = row_kth<W, kSmall>(rq, (int)mulhi32(rb, (uint32_t)nq));
+                        const bool led = (int)lq < W * 32 && row_has<W>(rq, (int)lq);
+                        if (close && led) a = (int)lq;
+                        if (match && led) {                    // same role as the replica that left `lo`
+                            if (moved_leader) a = (int)lq;
+                            else if (nq > 1) {
+                                uint32_t fol[W];
+#pragma unroll
+                                for (int t = 0; t < W; ++t) fol[t] = rq[t];
+                                row_flip<W>(fol, (int)lq);
+                                a = row_kth<W, kSmall>(fol, (int)mulhi32(rb, (uint32_t)(nq - 1)));
+                            }
+                        }
+                        o = olo;
+                    }
+                    moved_leader = (int)lq == a;
+                    const int moved_to = replace(rq, lq, a, o);
+                    if (link == 0) hi = moved_to; else lo = a;
+                } else {                                       // L-push / L-pull: one LEADER step
+                    int want = lo;
+                    if (link == 2 && !close) { const int h0 = d->homeT[q] & 0xFF; want = (h0 == 0xFF) ? -1 : h0; }
+                    const int old = (int)lq;
+                    const int t = pick_leader(rq, lq, want, rb);
+                    if (t < 0) return;
+                    if (link == 2) hi = t; else lo = old;
+                }
+                push(ps, q, rq, lq, rows);
+            }
+            return;
+        }
         for (int k = 1; k < nops; ++k) {
             const uint32_t link = (ctl >> (4 + 3 * (k - 1))) & 3u;
             const bool close = (ctl >> (6 + 3 * (k - 1))) & 1u;

@@ -28,6 +28,15 @@
     template __global__ void KAO_PERSISTENT_KERNEL_T(KAO_INST_W, 0, S, POP, T); \
     template __global__ void KAO_PERSISTENT_KERNEL_T(KAO_INST_W, 32, S, POP, T);
 KAO_FOR_SCHEDULES(KAO_INST_T)
+#if defined(KAO_PHASE_CLOCKS)
+// the phase probe's stamp buffer of this object's kernels (tools/time_phases.py; one symbol per translation unit)
+#define KAO_PHASE_BIND_NAME(W) kao_phase_clocks_bind_t##W
+#define KAO_PHASE_BIND(W) KAO_PHASE_BIND_NAME(W)
+extern "C" int KAO_PHASE_BIND(KAO_INST_W)(void *buf)
+{
+    return (int)cudaMemcpyToSymbol(kao_phase_buf, &buf, sizeof(buf));
+}
+#endif
 #elif KAO_INST_MODE == 1
 #if KAO_INST_W <= 2
 KAO_FOR_CFGS_NARROW(KAO_INST_DELTA_K, KAO_INST_W, KAO_INST_NPH)

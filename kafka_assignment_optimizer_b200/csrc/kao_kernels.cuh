@@ -31,7 +31,7 @@ template <class Cfg> constexpr int cfg_threads()
 // does a configuration form its sums on the tensor cores (column-major, kao_device_mma.cuh)
 template <class Cfg> __host__ __device__ constexpr bool cfg_mma()
 {
-    if constexpr (Cfg::kTrans) return Cfg::kSums == 1;
+    if constexpr (Cfg::kTrans) return Cfg::kSums >= 1;
     else return false;
 }
 
@@ -61,6 +61,24 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
                      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
     }
 }
+
+// Phase probe (tools/time_phases.py): a build with -DKAO_PHASE_CLOCKS records clock64 stamps of the persistent
+// search kernel into kao_phase_buf, [CTA][kPhaseWarps][kPhaseRounds][kPhaseSlots] u64, written by lane 0 of every
+// warp.  Without the flag KAO_PHASE(...) expands to nothing: the shipped kernels are compiled from the same tokens.
+#if defined(KAO_PHASE_CLOCKS)
+// per (CTA, warp, round): summed cycles of generate + park and of eval_batch_mma, the batches, and the stamps at the
+// round's start, after the warp's last batch, after the CTA reduce, the grid barrier, the winner's patch and rebuild_lists
+enum PhaseSlot { kPhGen, kPhEval, kPhBatches, kPhStart, kPhBatchesEnd, kPhReduce, kPhBarrier, kPhApply, kPhRebuild, kPhSlots };
+constexpr int kPhaseWarps = 32, kPhaseRounds = 64;
+static __device__ unsigned long long *kao_phase_buf;
+__device__ __forceinline__ unsigned long long *phase_rec(int warp, uint32_t t)
+{
+    return kao_phase_buf + (((size_t)blockIdx.x * kPhaseWarps + warp) * kPhaseRounds + t) * kPhSlots;
+}
+#define KAO_PHASE(...) __VA_ARGS__
+#else
+#define KAO_PHASE(...)
+#endif
 
 // Leader one-hot plane of the shared-memory base (kao_device.cuh, has_oh_plane): row & (1 << leader),
 // empty when the leader slot is not one of the row's replicas.  Stored right behind the bit-plane.
@@ -464,6 +482,9 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         const uint32_t round = first_round + t;
         gen.nD = s_counts[0]; gen.nL = s_counts[1];
         unsigned long long best = kKeyNone;
+        KAO_PHASE(unsigned long long *ph = (lane == 0 && t < kPhaseRounds) ? phase_rec(warp, t) : nullptr;
+                  unsigned long long ph_gen = 0, ph_eval = 0, ph_n = 0;
+                  if (ph) ph[kPhStart] = clock64();)
         if constexpr (kDelta) {
             // ---- delta mode: totals of the base once per round, then one THREAD per candidate
             const RoundTables rt = round_tables(smem, plan);
@@ -507,14 +528,16 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         } else if constexpr (cfg_mma<Cfg>()) {
             // ---- column-major evaluator, sums on the tensor cores (kao_device_mma.cuh): candidates are generated 32 at a
             // time, one per LANE, as below, then the warp evaluates all 32 together; lane (g, t) ends with the
-            // violation and objective of candidate mma_lane_candidate(lane) of the batch
-            Gen<W, true, true> tg;        // compact code (row_kth keeps its loop), same candidates
+            // violation and objective of candidate mma_lane_candidate(lane) of the batch.  Pop digit 2 = 2: the later
+            // operations' link kinds share their steps (Gen kMerged), same candidates
+            Gen<W, true, true, Cfg::kSums == 2> tg;        // compact code (row_kth keeps its loop), same candidates
             tg.bitsT = s_bits; tg.leader = s_leader; tg.cs = s_cs; tg.d = &d; tg.prow = nullptr; tg.lane = 0;
             tg.D = s_D; tg.DL = s_DL; tg.nD = s_counts[0]; tg.nL = s_counts[1];
             tg.T = s_sw; tg.tnW = t_words(d.Ppad); tg.t_leaders_valid = s_counts[2] == 0;    // "first holder of slot s": plane scan
             uint32_t *batch = s_prow + (size_t)warp * 32 * batch_stride<W>();
             const uint32_t j = (uint32_t)mma_lane_candidate(lane);
             for (uint32_t it0 = 0; it0 < iters; it0 += 32) {
+                KAO_PHASE(const unsigned long long ph0 = clock64();)
                 mma_clear_batch<W>(batch, lane);
                 __syncwarp();
                 {
@@ -534,8 +557,11 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                     mma_park_patch<W>(ps, rows, pviol, pobj, batch, lane);
                 }
                 __syncwarp();
+                KAO_PHASE(const unsigned long long ph1 = clock64();)
                 int viol, obj;
                 eval_batch_mma<Cfg>(d, s_cs, s_sw, t_words(d.Ppad), s_z, batch, lane, viol, obj);
+                KAO_PHASE(asm volatile("" ::"r"(viol), "r"(obj)); const unsigned long long ph2 = clock64();
+                          ph_gen += ph1 - ph0; ph_eval += ph2 - ph1; ++ph_n;)
                 const uint32_t idx = first + warp + (it0 + j) * stride;
                 if (it0 + j < iters && idx < pp.idx_hi) {
                     const unsigned long long key = pack_key(viol, obj, idx, d.key_obj_bits);
@@ -549,6 +575,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                 const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, best, o);
                 best = w < best ? w : best;
             }
+            KAO_PHASE(if (ph) { ph[kPhGen] = ph_gen; ph[kPhEval] = ph_eval; ph[kPhBatches] = ph_n; ph[kPhBatchesEnd] = clock64(); })
             if (all_keys) return;                                           // key dump only: the base stays as it is
         } else if constexpr (Cfg::kTrans) {
             // ---- column-major evaluator: candidates are generated 32 at a time, one per LANE (per-thread
@@ -634,6 +661,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         }
         if (lane == 0) s_red[warp] = best;
         __syncthreads();
+        KAO_PHASE(if (ph) ph[kPhReduce] = clock64();)
         if (warp == 0) {
             unsigned long long v = lane < kWarps ? s_red[lane] : kKeyNone;
 #pragma unroll
@@ -692,6 +720,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
             }
         }
         __syncthreads();
+        KAO_PHASE(if (ph) ph[kPhBarrier] = clock64();)
         if (s_abort) return;                                        // a peer vanished: leave, the host reports it
         // the winner becomes the base: every CTA patches its own shared-memory copy
         if (warp == 0) {
@@ -773,7 +802,9 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
             }
         }
         __syncthreads();
+        KAO_PHASE(if (ph) ph[kPhApply] = clock64();)
         rebuild_lists<THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
+        KAO_PHASE(if (ph) ph[kPhRebuild] = clock64();)
 #if !defined(KAO_NO_PATIENCE)
         if (s_red[kWarps]) break;
 #endif
@@ -797,9 +828,9 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // Column-major kernels: X(sync, pop, threads) for every built schedule (kao_set_schedule); each is
 // instantiated for W = 1, 2 and for 32 partition words (compile-time offsets) / any word count.
 #define KAO_FOR_SCHEDULES(X) \
-    X(1, 0x100, 512) X(4, 0x22, 1024) X(1, 0x22, 896) X(4, 0x22, 896) X(4, 0x12, 896) X(2, 0x22, 896)
+    X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896) X(4, 0x12, 896) X(2, 0x22, 896)
 #define KAO_SCHEDULE_DEFAULT_SYNC 1
-#define KAO_SCHEDULE_DEFAULT_POP 0x100
+#define KAO_SCHEDULE_DEFAULT_POP 0x200
 #define KAO_SCHEDULE_DEFAULT_THREADS 512
 #define KAO_PERSISTENT_KERNEL_T(W, NW, S, POP, T)                                                            \
     search_persistent_kernel<EvalCfgT<W, NW, S, POP, T>, T, false>(Params, SmemPlan, uint64_t, uint32_t, uint32_t, \
