@@ -43,13 +43,20 @@ extern "C" {
 #define KAO_MAX_ROUND_SIZE (1u << 24)
 #define KAO_MAX_ROUNDS (1u << 20)  /* rounds of one search call (one cooperative launch per 8192 when sharded) */
 #define KAO_MAX_GPUS 8
+#define KAO_MAX_PARTITIONS 65280      /* P: the largest multiple of 256 below 2^16 (u16 partition ids) */
+#define KAO_MAX_SMEM_PARTITIONS 8160  /* above this many partitions a session keeps its base in HBM (DESIGN.md 7.1) and
+                                         searches with delta evaluation only: kao_search, kao_candidate_keys (full
+                                         per-candidate evaluation, O(P * W) per candidate), kao_set_evaluator,
+                                         kao_set_schedule, KAO_FLAG_ROW_MAJOR, kao_profile_rounds and every sharded
+                                         entry point (kao_round_*, kao_p2p_*, kao_search_sharded*, kao_solve with
+                                         n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS) return KAO_E_ARG there */
 
 /*
  * The model, README.md:139-185.  x[b,p] / l[b,p] are the reference's binaries t1b{b}p{p} /
  * t1b{b}p{p}_l (README.md:146, :182-184); an assignment is exchanged as replica lists.
  */
 typedef struct kao_problem {
-    int32_t P;                /* partitions (rows; multi-topic input is flattened host-side) */
+    int32_t P;                /* partitions, 1..KAO_MAX_PARTITIONS (rows; multi-topic input is flattened host-side) */
     int32_t B;                /* brokers in the target list, README.md:48 */
     int32_t R;                /* racks / AZs, README.md:27-29 */
     int32_t RF;               /* target replication factor, C1 README.md:148-151 */
@@ -130,7 +137,9 @@ int kao_version(void);
 const char *kao_last_error(void);
 
 /* One blocking solve from host buffers: tables -> device, `rounds` search rounds, winner -> host.
- * Replaces "emit LP + run lp_solve + parse variables" (README.md:135-136, :139-185). */
+ * Replaces "emit LP + run lp_solve + parse variables" (README.md:135-136, :139-185).  Above KAO_MAX_SMEM_PARTITIONS
+ * partitions KAO_FLAG_DELTA is implied (the result is the assignment, whichever evaluator scored it); the options that
+ * path does not offer, and KAO_FLAG_LP_BOUND beyond the LP bound's limits, fail with KAO_E_ARG before any search. */
 int kao_solve(const kao_problem *pb, const kao_options *opt, kao_result *res);
 
 /* An upper bound on the objective of every feasible assignment of `pb` — what tells a caller how far a search
@@ -150,7 +159,8 @@ int kao_objective_bound(const kao_problem *pb, const int32_t *replicas, int64_t 
  * (1 .. KAO_MAX_LP_ITERATIONS).  bound = floor(min over the iterations of L / 2^KAO_LP_FRACTION_BITS); iterations_run =
  * evaluations of L; multipliers (optional, [2B + R]: C3 per broker, C4 per broker, C6 per rack) = the u of that
  * minimum.  The result is the same on every GPU and in every run.  KAO_E_ARG for an infeasible or malformed
- * assignment, KAO_E_CUDA without a device (there is no CPU path). */
+ * assignment, and beyond the build limits of MODEL §9 (P <= KAO_MAX_SMEM_PARTITIONS, P * RF < 2^16); KAO_E_CUDA
+ * without a device (there is no CPU path). */
 #define KAO_LP_FRACTION_BITS 20
 #define KAO_LP_ITERATIONS 4096              /* the cap kao_solve uses with KAO_FLAG_LP_BOUND */
 #define KAO_MAX_LP_ITERATIONS (1u << 20)
@@ -158,7 +168,8 @@ int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int32_t device,
                  int64_t *bound, uint32_t *iterations_run, int64_t *multipliers);
 
 /* Evaluate n explicit assignments (each [P*RF] replica lists, leader first, -1 padded) on the
- * GPU with the same evaluator the search uses: C1..C7 violation amount and objective. */
+ * GPU with the same evaluator the search uses: C1..C7 violation amount and objective.  (Above
+ * KAO_MAX_SMEM_PARTITIONS partitions: one CTA per assignment, per-row terms and per-slot totals.) */
 int kao_eval(const kao_problem *pb, int32_t device, const int32_t *replicas, int32_t n,
              int64_t *violation, int64_t *objective);
 
@@ -181,8 +192,8 @@ int kao_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t roun
 /* SURVEY.md 8(f)3 — the same search with DELTA evaluation: every candidate's key is derived from
  * the base's totals and its <= 3 patched rows (one thread per candidate) instead of a full pass
  * over its bit-plane.  Keys, winners and trajectory are bit-identical to kao_search; throughput
- * is reported separately (it is not the "full evaluation per candidate" metric).  Rows of up to 64
- * broker slots. */
+ * is reported separately (it is not the "full evaluation per candidate" metric).  Every row width; the only
+ * search above KAO_MAX_SMEM_PARTITIONS partitions (base in HBM, DESIGN.md 7.1). */
 int kao_search_delta(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds,
                      uint32_t round_size, uint64_t *round_keys, double *device_ms);
 int kao_candidate_keys_delta(kao_handle *h, uint64_t seed, uint32_t round, uint32_t round_size,

@@ -7,6 +7,7 @@
 #include "kao_host.hpp"
 #include "kao_bound.hpp"
 #include "kao_lagrange.hpp"
+#include "kao_large.hpp"
 #include "../../include/kao.h"
 
 #include <chrono>
@@ -216,6 +217,9 @@ struct kao_handle {
     uint64_t p2p_calls = 0;
     uint32_t patience = 0, last_rounds = 0;
     unsigned long long *d_lkeys = nullptr;   // kMailRounds keys, sharded search only
+    // more than kSmemRowsMax partitions (kao_large.cu): the base stays in HBM, delta search only
+    bool large = false;
+    LargeArgs la{};
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
 };
@@ -332,6 +336,11 @@ template <class F, class A> static cudaError_t dispatch(kao_handle *h, const F &
 // all rounds of a search in one cooperative launch, with the evaluator the session selected
 static cudaError_t launch_persistent(kao_handle *h, const PersistArgs &pa, bool delta)
 {
+    if (h->large) {
+        ++h->launches;
+        return large_search(h->hm.W, h->grid, h->prm, h->la, pa.seed, pa.first_round, pa.rounds, pa.round_size, pa.d_keys,
+                            pa.d_bar, pa.pp, pa.all_keys, pa.st);
+    }
     if (delta) return dispatch(h, LaunchPersistent<true>{}, pa);
     if (h->evaluator == KAO_EVAL_COLUMN_MAJOR) {
         const bool nw32 = h->hm.Ppad == 1024;                   // 32 partition words per slot: compile-time offsets
@@ -368,7 +377,8 @@ static int upload_base(kao_handle *h, const std::vector<uint32_t> &bitsT, const 
 {
     CUDA_TRY(cudaMemcpy(h->d_bits, bitsT.data(), bitsT.size() * 4, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(h->d_leader, leader.data(), leader.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(launch_apply(h, 0, 0, 2, h->d_key, /*regen_only=*/1, 0));
+    if (h->large) CUDA_TRY(large_prepare(h->hm.W, h->prm, h->la, 0));
+    else CUDA_TRY(launch_apply(h, 0, 0, 2, h->d_key, /*regen_only=*/1, 0));
     CUDA_TRY(cudaDeviceSynchronize());
     return KAO_OK;
 }
@@ -424,28 +434,35 @@ static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
     }
     const HostModel &m = h->hm;
     const int W = m.W, Ppad = m.Ppad;
-    h->threads = W <= 2 ? KAO_THREADS : KAO_THREADS_WIDE;
-    h->plan = make_plan(W, Ppad, h->threads / 32, m.nplanes > 0 ? m.nplanes * W : 4, m.P, m.RF, m.nplanes > 0);
-    if (h->plan.total > 227u * 1024u && m.nplanes > 0) {
-        // mask planes + one-hot plane do not fit next to the base: score with packed entries / the dense table
+    h->large = m.P > kSmemRowsMax;
+    if (h->large) {
+        // the large path scores the objective from packed entries or the dense table (no shared-memory planes)
         h->hm.nplanes = 0;
-        h->plan = make_plan(W, Ppad, h->threads / 32, 4, m.P, m.RF, false);
-    }
-    if (h->plan.total > 227u * 1024u)
-        return fail(KAO_E_ARG, "problem too large for the shared-memory resident search kernel");
-    // column-major evaluator: 8-slot rack fields, C7 = "at most one replica per rack", an objective that fits
-    // eight term planes (kao_host.hpp); its two transposed planes (2 * W words per partition) and the term planes
-    // take the place of the objective table.  It is the default full evaluator wherever it applies.
-    h->plan_t = make_plan_t(W, Ppad, KAO_THREADS, m.P, m.RF);
-    h->trans_ok = W <= 2 && m.hi1 && m.log2S == 3 && m.z_ok &&
-                  column_major_fits(W, Ppad, 1024, m.P, m.RF);     // incl. the inverted lists of its per-thread generator
-    if (h->trans_ok) h->evaluator = KAO_EVAL_COLUMN_MAJOR;
-    if (const char *env = std::getenv("KAO_EVALUATOR"))       // "row" forces the row-major evaluator (measurements)
-        if (std::strcmp(env, "row") == 0) h->evaluator = KAO_EVAL_ROW_MAJOR;
-    if (const char *env = std::getenv("KAO_SCHEDULE")) {      // "sync,pop(hex),threads": measurements only, ignored if not built
-        int a = 0, c = 0; unsigned b = 0;
-        if (std::sscanf(env, "%d,%x,%d", &a, &b, &c) == 3 && schedule_exists(a, (int)b, c)) {
-            h->sch_sync = a; h->sch_pop = (int)b; h->sch_threads = c;
+        h->hm.z_ok = false;
+    } else {
+        h->threads = W <= 2 ? KAO_THREADS : KAO_THREADS_WIDE;
+        h->plan = make_plan(W, Ppad, h->threads / 32, m.nplanes > 0 ? m.nplanes * W : 4, m.P, m.RF, m.nplanes > 0);
+        if (h->plan.total > 227u * 1024u && m.nplanes > 0) {
+            // mask planes + one-hot plane do not fit next to the base: score with packed entries / the dense table
+            h->hm.nplanes = 0;
+            h->plan = make_plan(W, Ppad, h->threads / 32, 4, m.P, m.RF, false);
+        }
+        if (h->plan.total > 227u * 1024u)
+            return fail(KAO_E_ARG, "problem too large for the shared-memory resident search kernel");
+        // column-major evaluator: 8-slot rack fields, C7 = "at most one replica per rack", an objective that fits
+        // eight term planes (kao_host.hpp); its two transposed planes (2 * W words per partition) and the term planes
+        // take the place of the objective table.  It is the default full evaluator wherever it applies.
+        h->plan_t = make_plan_t(W, Ppad, KAO_THREADS, m.P, m.RF);
+        h->trans_ok = W <= 2 && m.hi1 && m.log2S == 3 && m.z_ok &&
+                      column_major_fits(W, Ppad, 1024, m.P, m.RF);     // incl. the inverted lists of its per-thread generator
+        if (h->trans_ok) h->evaluator = KAO_EVAL_COLUMN_MAJOR;
+        if (const char *env = std::getenv("KAO_EVALUATOR"))       // "row" forces the row-major evaluator (measurements)
+            if (std::strcmp(env, "row") == 0) h->evaluator = KAO_EVAL_ROW_MAJOR;
+        if (const char *env = std::getenv("KAO_SCHEDULE")) {      // "sync,pop(hex),threads": measurements only, ignored if not built
+            int a = 0, c = 0; unsigned b = 0;
+            if (std::sscanf(env, "%d,%x,%d", &a, &b, &c) == 3 && schedule_exists(a, (int)b, c)) {
+                h->sch_sync = a; h->sch_pop = (int)b; h->sch_threads = c;
+            }
         }
     }
     h->grid = h->sms;
@@ -453,8 +470,15 @@ static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
     CUDA_TRY(dalloc(h, &h->d_leader, (size_t)Ppad));
     CUDA_TRY(dalloc(h, &h->d_sw, (size_t)4 * Ppad * 4));
     CUDA_TRY(dalloc(h, &h->d_home, (size_t)Ppad * 4));
-    CUDA_TRY(dalloc(h, &h->d_D, (size_t)Ppad * 2));
-    CUDA_TRY(dalloc(h, &h->d_DL, (size_t)Ppad * 2));
+    // the large path keeps two buffers per displaced list (kao_large.hpp), its transposed planes and winner record
+    const size_t nlists = h->large ? 2 : 1;
+    CUDA_TRY(dalloc(h, &h->d_D, nlists * Ppad * 2));
+    CUDA_TRY(dalloc(h, &h->d_DL, nlists * Ppad * 2));
+    if (h->large) {
+        h->la.tnW = t_words(Ppad);
+        CUDA_TRY(dalloc(h, &h->la.T, (size_t)kTPlanes * 32 * W * h->la.tnW * 4));
+        CUDA_TRY(dalloc(h, &h->la.rec, sizeof(LargeRecord)));
+    }
     CUDA_TRY(dalloc(h, &h->d_nD, 16));
     CUDA_TRY(dalloc(h, &h->d_consts, sizeof(Consts)));
     CUDA_TRY(dalloc(h, &h->d_key, 16));
@@ -518,6 +542,11 @@ static int set_base_impl(kao_handle *h, const int32_t *replicas)
 static int eval_on_device(kao_handle *h, const uint32_t *d_bits, const uint8_t *d_leader, int n,
                           long long *d_viol, long long *d_obj)
 {
+    if (h->large) {
+        CUDA_TRY(large_eval(h->hm.W, h->prm, d_bits, d_leader, n, d_viol, d_obj, 0));
+        ++h->launches;
+        return KAO_OK;
+    }
     const int blocks = (n * 32 + 255) / 256;
     with_row_width(h->hm.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
@@ -554,6 +583,18 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
     return KAO_OK;
 }
 
+// what a session of more than kSmemRowsMax partitions does not offer (kao.h): full per-candidate evaluation, the choice
+// of full evaluator, and sharding one search over several GPUs
+static int refuse_large(const char *what)
+{
+    return fail(KAO_E_ARG, std::string(what) + ": not offered above 8,160 partitions (the base of those kernels is "
+                                               "staged in shared memory); larger problems are searched with delta "
+                                               "evaluation on one GPU per search");
+}
+// the build limits of the Lagrangian LP bound (docs/MODEL.md §9)
+static bool lp_bound_fits(const kao_problem &pb) { return pb.P <= kSmemRowsMax && (int64_t)pb.P * pb.RF < 65536; }
+static const char *kLpLimit = "the Lagrangian LP bound is built for P <= 8,160 and P * RF < 2^16 (docs/MODEL.md 9)";
+
 static bool check_round_args(uint32_t round_size) { return round_size >= 2 && round_size <= KAO_MAX_ROUND_SIZE; }
 // delta evaluation keeps the base and the per-round tables in shared memory (rows wider than 64 slots: without the objective table)
 static bool delta_fits(const kao_handle *h)
@@ -565,9 +606,12 @@ static bool delta_fits(const kao_handle *h)
 // yet (h == nullptr): each of its sessions checks delta evaluation again when it searches
 static int check_search_args(const kao_handle *h, uint32_t rounds, uint32_t round_size, bool delta)
 {
+    if (h && h->large && !delta)
+        return fail(KAO_E_ARG, "full per-candidate evaluation is not offered above 8,160 partitions: use delta evaluation "
+                               "(kao_search_delta, kao_candidate_keys_delta)");
     if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
-    if (delta && h && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
+    if (delta && h && !h->large && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
     return KAO_OK;
 }
 
@@ -610,7 +654,8 @@ static int timed_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint
     CUDA_TRY(cudaEventRecord(h->ev0, 0));
     if (rounds) {
         if ((rc = launch_rounds()) != KAO_OK) return rc;
-        CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
+        // the large path keeps the displaced lists in HBM current itself
+        if (!h->large) CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
     }
     CUDA_TRY(cudaEventRecord(h->ev1, 0));
     CUDA_TRY(cudaEventSynchronize(h->ev1));
@@ -700,6 +745,7 @@ static int publish_mailboxes(kao_handle *h, int rank, int world)
 static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 {
     if (!h || !handle_out) return fail(KAO_E_ARG, "null argument");
+    if (h->large) return refuse_large("kao_p2p_export");
     static_assert(sizeof(cudaIpcMemHandle_t) == KAO_IPC_HANDLE_BYTES, "ipc handle size");
     const int rc = ensure_mailbox(h);
     if (rc != KAO_OK) return rc;
@@ -712,6 +758,7 @@ static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 static int p2p_connect_impl(kao_handle *h, int32_t rank, int32_t world, const uint8_t *handles)
 {
     if (!h || !handles) return fail(KAO_E_ARG, "null argument");
+    if (h->large) return refuse_large("kao_p2p_connect");
     if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(KAO_E_ARG, "bad rank / world");
     if (!h->d_mail) return fail(KAO_E_STATE, "call kao_p2p_export first");
     CUDA_TRY(cudaSetDevice(h->device));
@@ -731,6 +778,7 @@ static int sharded_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint
                         uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
 {
     if (!h) return fail(KAO_E_ARG, "null handle");
+    if (h->large) return refuse_large("sharded search");
     const int rc = check_search_args(h, rounds, round_size, delta);
     if (rc != KAO_OK) return rc;
     if (h->p2p_world < 2 || !h->peer_mail[h->p2p_world - 1]) return fail(KAO_E_STATE, "kao_p2p_connect first");
@@ -776,6 +824,7 @@ static int profile_rounds_impl(kao_handle *h, uint64_t seed, uint32_t first_roun
                                uint32_t round_size, double *search_ms, double *apply_ms)
 {
     if (!h || !rounds || rounds > 4096) return fail(KAO_E_ARG, "bad argument (1..4096 rounds)");
+    if (h->large) return refuse_large("kao_profile_rounds (full evaluation, one launch per round)");
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
     CUDA_TRY(cudaSetDevice(h->device));
     struct Events {
@@ -1096,6 +1145,13 @@ static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result 
     if (!pb || !opt || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
     int rc = check_search_args(nullptr, opt->rounds, opt->round_size, false);
     if (rc != KAO_OK) return rc;
+    // more than kSmemRowsMax partitions: the large path, which searches with delta evaluation (kao_solve returns the
+    // assignment, whatever evaluator found it) on one GPU per search; refused before anything is searched
+    const bool large = pb->P > kSmemRowsMax;
+    const bool sharded = (opt->n_gpus > 1 || __builtin_popcount(opt->device_mask) > 1) && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS);
+    if (large && (opt->flags & KAO_FLAG_ROW_MAJOR)) return refuse_large("KAO_FLAG_ROW_MAJOR");
+    if (large && sharded) return refuse_large("n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS (every round sharded over the GPUs)");
+    if ((opt->flags & KAO_FLAG_LP_BOUND) && !lp_bound_fits(*pb)) return fail(KAO_E_ARG, std::string("KAO_FLAG_LP_BOUND: ") + kLpLimit);
     const auto t0 = std::chrono::steady_clock::now();
     std::vector<int> devs;
     rc = pick_devices(opt, devs);
@@ -1104,7 +1160,7 @@ static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result 
     // independent restarts (flags & 0xFF, 0 and 1 both mean a single search): each restarts from the
     // initial base with its own seed; the best final assignment wins (better())
     const uint32_t restarts = (opt->flags & 0xFFu) ? (opt->flags & 0xFFu) : 1u;
-    const bool delta = (opt->flags & KAO_FLAG_DELTA) != 0;
+    const bool delta = (opt->flags & KAO_FLAG_DELTA) != 0 || large;
     Solved s;
     rc = world > 1 && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS) ? solve_gang(pb, opt, devs, restarts, delta, s)
                                                                 : solve_restarts(pb, opt, devs, restarts, delta, t0, s);
@@ -1177,6 +1233,7 @@ extern "C" int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int3
         HostModel m;
         std::string why;
         if (!build_host_model(*pb, m, why)) return fail(KAO_E_ARG, why);
+        if (!lp_bound_fits(*pb)) return fail(KAO_E_ARG, std::string("kao_lp_bound: ") + kLpLimit);
         int64_t T = 0;
         if (!feasible_objective(*pb, replicas, T, why)) return fail(KAO_E_ARG, why);
         int ndev = 0;
@@ -1199,6 +1256,7 @@ extern "C" int kao_round_launch(kao_handle *h, uint64_t seed, uint32_t round, ui
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
+        if (h->large) return refuse_large("kao_round_launch");
         if (!check_round_args(round_size) || idx_lo > idx_hi || idx_hi > round_size)
             return fail(KAO_E_ARG, "bad round_size / index range");
         CUDA_TRY(cudaSetDevice(h->device));
@@ -1212,6 +1270,7 @@ extern "C" int kao_round_apply(kao_handle *h, uint64_t seed, uint32_t round, uin
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
+        if (h->large) return refuse_large("kao_round_apply");
         if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
         CUDA_TRY(cudaSetDevice(h->device));
         CUDA_TRY(launch_apply(h, seed, round, round_size, reinterpret_cast<const unsigned long long *>(d_key), 0,
@@ -1223,6 +1282,7 @@ extern "C" int kao_set_evaluator(kao_handle *h, int32_t evaluator)
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
+        if (h->large) return refuse_large("kao_set_evaluator");
         if (evaluator != KAO_EVAL_ROW_MAJOR && evaluator != KAO_EVAL_COLUMN_MAJOR) return fail(KAO_E_ARG, "unknown evaluator");
         if (evaluator == KAO_EVAL_COLUMN_MAJOR && !h->trans_ok)
             return fail(KAO_E_ARG, "column-major evaluator: needs rows of up to 64 slots, racks of up to 8 brokers, at most one "
@@ -1235,6 +1295,7 @@ extern "C" int kao_set_schedule(kao_handle *h, int32_t sync, int32_t pop, int32_
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
+        if (h->large) return refuse_large("kao_set_schedule");
         if (!schedule_exists(sync, pop, threads)) return fail(KAO_E_ARG, "no such schedule (kao.h, kao_set_schedule)");
         h->sch_sync = sync; h->sch_pop = pop; h->sch_threads = threads;
         return KAO_OK;

@@ -50,7 +50,9 @@ struct HostModel {
 inline bool build_host_model(const kao_problem &pb, HostModel &m, std::string &why)
 {
     auto bad = [&](const char *s) { why = s; return false; };
-    if (pb.P < 1 || pb.P > 8160) return bad("P must be 1..8160");
+    // 65,280: the largest multiple of 256 below 2^16 (u16 partition ids and their 0xFFFF sentinel); above 8,160
+    // partitions the engine searches with the base in HBM (kao_large.cu)
+    if (pb.P < 1 || pb.P > 65280) return bad("P must be 1..65280");
     if (pb.B < 2 || pb.B > KAO_MAX_SLOTS) return bad("B must be 2..256");
     if (pb.R < 1 || pb.R > KAO_MAX_RACKS) return bad("R must be 1..32");
     if (pb.RF < 1 || pb.RF > KAO_MAX_RF || pb.RF >= pb.B) return bad("RF must be 1..8 and < B");
