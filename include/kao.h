@@ -167,6 +167,27 @@ int kao_objective_bound(const kao_problem *pb, const int32_t *replicas, int64_t 
 int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int32_t device, uint32_t max_iterations,
                  int64_t *bound, uint32_t *iterations_run, int64_t *multipliers);
 
+/*
+ * Per-topic balance rows (docs/MODEL.md §10).  The balance rows of README.md:158-166 sum over ONE topic's
+ * partitions; kao_problem flattens every topic into rows, so C3 / C4 bound cluster-wide totals only.  A kao_topics
+ * ADDS, for every topic t and broker b:
+ *   C3t  rep_lo[t] <= replicas of topic t's partitions on b        <= rep_hi[t]
+ *   C4t  ldr_lo[t] <= partitions of topic t led (validly) from b   <= ldr_hi[t]
+ * to the violation; every other row, the objective and the candidate stream stay as they are.  Valid input:
+ * 1 <= T <= P, 0 <= topic_of[p] < T, 0 <= lo <= hi, rep_lo[t] <= n_t * RF and ldr_lo[t] <= n_t (n_t = partitions of
+ * topic t); anything else is KAO_E_ARG before any CUDA call.  The defaults of the Python binding (topic_rows) are
+ * floor / ceil of n_t * RF / B and n_t / B.
+ */
+typedef struct kao_topics {
+    int32_t T;                  /* topics */
+    const int32_t *topic_of;    /* [P] topic of each partition */
+    const int32_t *rep_lo, *rep_hi;   /* [T] C3t */
+    const int32_t *ldr_lo, *ldr_hi;   /* [T] C4t */
+} kao_topics;
+
+/* kao_solve with the topic rows of `tp` (tp == NULL: exactly kao_solve); see kao_create_topics */
+int kao_solve_topics(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, kao_result *res);
+
 /* Evaluate n explicit assignments (each [P*RF] replica lists, leader first, -1 padded) on the
  * GPU with the same evaluator the search uses: C1..C7 violation amount and objective.  (Above
  * KAO_MAX_SMEM_PARTITIONS partitions: one CTA per assignment, per-row terms and per-slot totals.) */
@@ -177,6 +198,14 @@ int kao_eval(const kao_problem *pb, int32_t device, const int32_t *replicas, int
 typedef struct kao_handle kao_handle;
 
 int kao_create(const kao_problem *pb, int32_t device, kao_handle **out);
+/* kao_create with the topic rows of `tp` (tp == NULL: exactly kao_create).  A topic session keeps its base in HBM at
+ * every P (DESIGN.md 7.2) and searches by delta evaluation (KAO_FLAG_DELTA implied); what a session above
+ * KAO_MAX_SMEM_PARTITIONS refuses, it refuses at any P (KAO_E_ARG).  kao_search_delta, kao_candidate_keys_delta,
+ * kao_set_base, kao_get_base (the violation includes the topic rows), patience, restarts and KAO_FLAG_SPREAD_RESTARTS
+ * work as on any session.  KAO_FLAG_BOUND / KAO_FLAG_LP_BOUND bound the problem WITHOUT the topic rows: still an upper
+ * bound (the topic rows only remove assignments), possibly a looser one; optimal = 1 still means proven.  Device
+ * memory: 4 bytes per (topic, slot) for the counts (67 MB at 65,280 topics x 256 slots). */
+int kao_create_topics(const kao_problem *pb, const kao_topics *tp, int32_t device, kao_handle **out);
 int kao_destroy(kao_handle *h);
 /* base <- current assignment restricted to the target brokers and completed to RF (MODEL §4) */
 int kao_reset(kao_handle *h);

@@ -114,6 +114,9 @@ struct Model {
     std::vector<int32_t> rep_lo, rep_hi, ldr_lo, ldr_hi, rack_lo, rack_hi, cur;
     int ppr_lo = 0, ppr_hi = 0;
     std::vector<Row> rows;
+    // per-topic rows (docs/MODEL.md §10, --topic-balance): topics in name order, floor / ceil of n_t * RF / B and n_t / B
+    std::vector<std::string> topic_names;
+    std::vector<int32_t> topic_of, trep_lo, trep_hi, tldr_lo, tldr_hi;
 };
 
 static int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
@@ -165,11 +168,21 @@ Model build_model(std::vector<Row> rows, std::vector<int> brokers, const std::ma
         m.rack_hi.push_back(ceil_div(tot * size[r], m.B));
     }
     m.ppr_lo = rf / m.R; m.ppr_hi = ceil_div(rf, m.R);                                        // README.md:178-180
+    std::vector<long> n;
+    for (const Row &r : m.rows) {                               // rows are sorted by topic: a new name starts a topic
+        if (m.topic_names.empty() || m.topic_names.back() != r.topic) { m.topic_names.push_back(r.topic); n.push_back(0); }
+        m.topic_of.push_back((int32_t)m.topic_names.size() - 1);
+        ++n.back();
+    }
+    for (long nt : n) {
+        m.trep_lo.push_back((int)(nt * rf / m.B)); m.trep_hi.push_back(ceil_div(nt * rf, m.B));
+        m.tldr_lo.push_back((int)(nt / m.B));      m.tldr_hi.push_back(ceil_div(nt, m.B));
+    }
     return m;
 }
 
 // lp_solve LP-format text, same families and naming as README.md:144-185
-void emit_lp(const Model &m, std::ostream &o)
+void emit_lp(const Model &m, std::ostream &o, bool topics)
 {
     auto var = [&](int b, int p, bool l) {
         return "t1b" + std::to_string(m.broker_ids[b]) + "p" + std::to_string(p) + (l ? "_l" : "");
@@ -229,6 +242,23 @@ void emit_lp(const Model &m, std::ostream &o)
                 }
                 o << (pass ? " >= " : " <= ") << (pass ? m.ppr_lo : m.ppr_hi) << ";\n";
             }
+    for (int t = 0; topics && t < (int)m.topic_names.size(); ++t)
+        for (int kind = 0; kind < 2; ++kind) {
+            o << "\n// Constraint on min/max " << (kind ? "leaders" : "replicas") << " of topic " << m.topic_names[t]
+              << " per broker\n";
+            for (int b = 0; b < m.B; ++b)
+                for (int pass = 0; pass < 2; ++pass) {
+                    bool f2 = true;
+                    for (int p = 0; p < m.P; ++p) {
+                        if (m.topic_of[p] != t) continue;
+                        if (!kind) o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true);
+                        else o << (f2 ? "" : " + ") << var(b, p, true);
+                        f2 = false;
+                    }
+                    const int lo = kind ? m.tldr_lo[t] : m.trep_lo[t], hi = kind ? m.tldr_hi[t] : m.trep_hi[t];
+                    o << (pass ? " >= " : " <= ") << (pass ? lo : hi) << ";\n";
+                }
+        }
     o << "\n// All variables are binary\nbin\n";
     for (int p = 0; p < m.P; ++p)
         for (int b = 0; b < m.B; ++b)
@@ -258,7 +288,7 @@ int usage()
 {
     std::fprintf(stderr,
                  "usage: kao-cli --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
-                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--emit-lp] [--stats]\n");
+                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--topic-balance] [--emit-lp] [--stats]\n");
     return 2;
 }
 
@@ -267,7 +297,8 @@ int usage()
 int main(int argc, char **argv)
 {
     std::map<std::string, std::string> a;
-    bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false, lp_certificate = false;
+    bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false, lp_certificate = false,
+         topic_balance = false;
     for (int i = 1; i < argc; ++i) {
         std::string k = argv[i];
         if (k == "--emit-lp") { emit = true; continue; }
@@ -277,6 +308,7 @@ int main(int argc, char **argv)
         if (k == "--spread-restarts") { spread = true; continue; }   // --gpus N: the restarts side by side, one per GPU at a time
         if (k == "--certificate") { certificate = true; continue; }  // flow bound: --stats can then say "proven optimal"
         if (k == "--lp-certificate") { lp_certificate = true; continue; }  // Lagrangian LP bound (GPU): proves what the flow bound cannot
+        if (k == "--topic-balance") { topic_balance = true; continue; }   // every topic spread over the brokers too
         if (k == "--column-major") continue;                  // accepted for old scripts: it is the default now
         if (k.rfind("--", 0) != 0 || i + 1 >= argc) return usage();
         a[k.substr(2)] = argv[++i];
@@ -307,7 +339,7 @@ int main(int argc, char **argv)
         for (auto &r : rows) rf = std::max(rf, (int)r.replicas.size());
         if (a.count("rf")) rf = std::atoi(a["rf"].c_str());
         Model m = build_model(rows, brokers, racks, rf);
-        if (emit) { emit_lp(m, std::cout); return 0; }
+        if (emit) { emit_lp(m, std::cout, topic_balance); return 0; }
 
         kao_problem pb{};
         pb.P = m.P; pb.B = m.B; pb.R = m.R; pb.RF = m.RF; pb.RFcur = m.RFcur;
@@ -331,7 +363,9 @@ int main(int argc, char **argv)
         std::vector<int32_t> reps((size_t)m.P * m.RF, -1);
         kao_result res{};
         res.replicas = reps.data();
-        const int rc = kao_solve(&pb, &opt, &res);
+        kao_topics tp{(int32_t)m.topic_names.size(), m.topic_of.data(), m.trep_lo.data(), m.trep_hi.data(),
+                      m.tldr_lo.data(), m.tldr_hi.data()};
+        const int rc = topic_balance ? kao_solve_topics(&pb, &tp, &opt, &res) : kao_solve(&pb, &opt, &res);
         if (rc < 0) { std::fprintf(stderr, "kao-cli: %s\n", kao_last_error()); return 1; }
         if (rc == KAO_INFEASIBLE)
             std::fprintf(stderr, "kao-cli: warning: no assignment satisfying every constraint was found (violation %lld)\n",

@@ -220,6 +220,9 @@ struct kao_handle {
     // more than kSmemRowsMax partitions (kao_large.cu): the base stays in HBM, delta search only
     bool large = false;
     LargeArgs la{};
+    // per-topic balance rows (kao_create_topics): always on the large path
+    bool topics = false;
+    TopicArgs ta{};
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
 };
@@ -339,7 +342,7 @@ static cudaError_t launch_persistent(kao_handle *h, const PersistArgs &pa, bool 
     if (h->large) {
         ++h->launches;
         return large_search(h->hm.W, h->grid, h->prm, h->la, pa.seed, pa.first_round, pa.rounds, pa.round_size, pa.d_keys,
-                            pa.d_bar, pa.pp, pa.all_keys, pa.st);
+                            pa.d_bar, pa.pp, pa.all_keys, pa.st, h->topics ? &h->ta : nullptr);
     }
     if (delta) return dispatch(h, LaunchPersistent<true>{}, pa);
     if (h->evaluator == KAO_EVAL_COLUMN_MAJOR) {
@@ -379,6 +382,7 @@ static int upload_base(kao_handle *h, const std::vector<uint32_t> &bitsT, const 
     CUDA_TRY(cudaMemcpy(h->d_leader, leader.data(), leader.size(), cudaMemcpyHostToDevice));
     if (h->large) CUDA_TRY(large_prepare(h->hm.W, h->prm, h->la, 0));
     else CUDA_TRY(launch_apply(h, 0, 0, 2, h->d_key, /*regen_only=*/1, 0));
+    if (h->topics) CUDA_TRY(topics_prepare(h->hm.W, h->prm, h->ta, 0));
     CUDA_TRY(cudaDeviceSynchronize());
     return KAO_OK;
 }
@@ -416,10 +420,12 @@ static int reset_impl(kao_handle *h)
     return upload_base(h, bitsT, leader);
 }
 
-static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
+static int create_impl(const kao_problem *pb, const kao_topics *tp, int32_t device, kao_handle *h)
 {
     std::string why;
     if (!build_host_model(*pb, h->hm, why)) return fail(KAO_E_ARG, why);
+    HostTopics ht;
+    if (tp && !build_host_topics(*pb, *tp, h->hm.Ppad, ht, why)) return fail(KAO_E_ARG, why);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
         return fail(KAO_E_CUDA, "no CUDA device: libkao has no CPU path");
@@ -434,7 +440,8 @@ static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
     }
     const HostModel &m = h->hm;
     const int W = m.W, Ppad = m.Ppad;
-    h->large = m.P > kSmemRowsMax;
+    h->topics = tp != nullptr;
+    h->large = m.P > kSmemRowsMax || h->topics;
     if (h->large) {
         // the large path scores the objective from packed entries or the dense table (no shared-memory planes)
         h->hm.nplanes = 0;
@@ -479,6 +486,23 @@ static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
         CUDA_TRY(dalloc(h, &h->la.T, (size_t)kTPlanes * 32 * W * h->la.tnW * 4));
         CUDA_TRY(dalloc(h, &h->la.rec, sizeof(LargeRecord)));
     }
+    if (h->topics) {
+        // topic of each partition, bounds per topic, replica and leader counts per (topic, slot), the base's violation
+        TopicArgs &ta = h->ta;
+        const size_t cells = (size_t)ht.T * 32 * W;
+        uint16_t *topic_of = nullptr;
+        int4 *bnd = nullptr;
+        ta.T = ht.T;
+        CUDA_TRY(dalloc(h, &topic_of, ht.topic_of.size() * 2));
+        CUDA_TRY(dalloc(h, &bnd, (size_t)ht.T * sizeof(int4)));
+        CUDA_TRY(dalloc(h, &ta.tcnt, cells * 2));
+        CUDA_TRY(dalloc(h, &ta.tlcnt, cells * 2));
+        CUDA_TRY(dalloc(h, &ta.tviol, 16));
+        CUDA_TRY(cudaMemcpy(topic_of, ht.topic_of.data(), ht.topic_of.size() * 2, cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(bnd, ht.bnd.data(), ht.bnd.size() * 4, cudaMemcpyHostToDevice));
+        ta.topic_of = topic_of;
+        ta.bnd = bnd;
+    }
     CUDA_TRY(dalloc(h, &h->d_nD, 16));
     CUDA_TRY(dalloc(h, &h->d_consts, sizeof(Consts)));
     CUDA_TRY(dalloc(h, &h->d_key, 16));
@@ -519,13 +543,13 @@ static int create_impl(const kao_problem *pb, int32_t device, kao_handle *h)
     return reset_impl(h);
 }
 
-static int create_handle(const kao_problem *pb, int32_t device, kao_handle **out)
+static int create_handle(const kao_problem *pb, int32_t device, kao_handle **out, const kao_topics *tp = nullptr)
 {
     if (!pb || !out) return fail(KAO_E_ARG, "null argument");
     *out = nullptr;
     HandleOwner s;
     s.h = new kao_handle();
-    const int rc = create_impl(pb, device, s.h);
+    const int rc = create_impl(pb, tp, device, s.h);
     if (rc == KAO_OK) { *out = s.h; s.h = nullptr; }
     return rc;
 }
@@ -573,7 +597,13 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
     if (moves) *moves = count_moves(m, reps.data());
     if (violation || objective) {
         if (!h->d_vo) CUDA_TRY(dalloc(h, &h->d_vo, 16));
-        int rc = eval_on_device(h, h->d_bits, h->d_leader, 1, h->d_vo, h->d_vo + 1);
+        int rc = KAO_OK;
+        if (h->topics) {
+            CUDA_TRY(large_eval_topics(h->hm.W, h->prm, h->ta, h->d_vo, h->d_vo + 1, 0));
+            ++h->launches;
+        } else {
+            rc = eval_on_device(h, h->d_bits, h->d_leader, 1, h->d_vo, h->d_vo + 1);
+        }
         long long vo[2] = {0, 0};
         if (rc == KAO_OK && cudaMemcpy(vo, h->d_vo, 16, cudaMemcpyDeviceToHost) != cudaSuccess) rc = KAO_E_CUDA;
         if (rc != KAO_OK) return rc;
@@ -585,8 +615,12 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
 
 // what a session of more than kSmemRowsMax partitions does not offer (kao.h): full per-candidate evaluation, the choice
 // of full evaluator, and sharding one search over several GPUs
-static int refuse_large(const char *what)
+static int refuse_large(const char *what, bool topics = false)
 {
+    if (topics)
+        return fail(KAO_E_ARG, std::string(what) + ": not offered with topic rows (kao_create_topics / kao_solve_topics "
+                                                   "keep the base and the per-topic counts in HBM and search with delta "
+                                                   "evaluation on one GPU per search, at every P)");
     return fail(KAO_E_ARG, std::string(what) + ": not offered above 8,160 partitions (the base of those kernels is "
                                                "staged in shared memory); larger problems are searched with delta "
                                                "evaluation on one GPU per search");
@@ -607,8 +641,9 @@ static bool delta_fits(const kao_handle *h)
 static int check_search_args(const kao_handle *h, uint32_t rounds, uint32_t round_size, bool delta)
 {
     if (h && h->large && !delta)
-        return fail(KAO_E_ARG, "full per-candidate evaluation is not offered above 8,160 partitions: use delta evaluation "
-                               "(kao_search_delta, kao_candidate_keys_delta)");
+        return fail(KAO_E_ARG, std::string("full per-candidate evaluation is not offered ") +
+                                   (h->topics ? "with topic rows" : "above 8,160 partitions") +
+                                   ": use delta evaluation (kao_search_delta, kao_candidate_keys_delta)");
     if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
     if (delta && h && !h->large && !delta_fits(h)) return fail(KAO_E_ARG, "delta evaluation: the base and its per-round tables do not fit in shared memory");
@@ -745,7 +780,7 @@ static int publish_mailboxes(kao_handle *h, int rank, int world)
 static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 {
     if (!h || !handle_out) return fail(KAO_E_ARG, "null argument");
-    if (h->large) return refuse_large("kao_p2p_export");
+    if (h->large) return refuse_large("kao_p2p_export", h->topics);
     static_assert(sizeof(cudaIpcMemHandle_t) == KAO_IPC_HANDLE_BYTES, "ipc handle size");
     const int rc = ensure_mailbox(h);
     if (rc != KAO_OK) return rc;
@@ -758,7 +793,7 @@ static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 static int p2p_connect_impl(kao_handle *h, int32_t rank, int32_t world, const uint8_t *handles)
 {
     if (!h || !handles) return fail(KAO_E_ARG, "null argument");
-    if (h->large) return refuse_large("kao_p2p_connect");
+    if (h->large) return refuse_large("kao_p2p_connect", h->topics);
     if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(KAO_E_ARG, "bad rank / world");
     if (!h->d_mail) return fail(KAO_E_STATE, "call kao_p2p_export first");
     CUDA_TRY(cudaSetDevice(h->device));
@@ -778,7 +813,7 @@ static int sharded_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint
                         uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
 {
     if (!h) return fail(KAO_E_ARG, "null handle");
-    if (h->large) return refuse_large("sharded search");
+    if (h->large) return refuse_large("sharded search", h->topics);
     const int rc = check_search_args(h, rounds, round_size, delta);
     if (rc != KAO_OK) return rc;
     if (h->p2p_world < 2 || !h->peer_mail[h->p2p_world - 1]) return fail(KAO_E_STATE, "kao_p2p_connect first");
@@ -824,7 +859,7 @@ static int profile_rounds_impl(kao_handle *h, uint64_t seed, uint32_t first_roun
                                uint32_t round_size, double *search_ms, double *apply_ms)
 {
     if (!h || !rounds || rounds > 4096) return fail(KAO_E_ARG, "bad argument (1..4096 rounds)");
-    if (h->large) return refuse_large("kao_profile_rounds (full evaluation, one launch per round)");
+    if (h->large) return refuse_large("kao_profile_rounds (full evaluation, one launch per round)", h->topics);
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
     CUDA_TRY(cudaSetDevice(h->device));
     struct Events {
@@ -1100,15 +1135,15 @@ static int solve_gang(const kao_problem *pb, const kao_options *opt, const std::
 // The restarts side by side on the GPUs of the call: restart r runs on GPU r mod N as an ordinary single-GPU search
 // (no exchange between the GPUs at all), one host thread per GPU and none for one GPU.  The winner is exactly what
 // one GPU returns for the same call: this is kao_solve on one GPU, and with KAO_FLAG_SPREAD_RESTARTS on several.
-static int solve_restarts(const kao_problem *pb, const kao_options *opt, const std::vector<int> &devs, uint32_t restarts,
-                          bool delta, std::chrono::steady_clock::time_point t0, Solved &out)
+static int solve_restarts(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, const std::vector<int> &devs,
+                          uint32_t restarts, bool delta, std::chrono::steady_clock::time_point t0, Solved &out)
 {
     const int world = (int)devs.size();
     std::vector<Solved> per(world);
     const int rc = on_each_gpu(devs, [&](int i) {
         Solved &g = per[i];
         HandleOwner s;
-        int rc = create_handle(pb, devs[i], &s.h);
+        int rc = create_handle(pb, devs[i], &s.h, tp);
         if (rc != KAO_OK) return rc;
         stamp(t0, "session created (model built, tables uploaded, initial base)");
         kao_handle *h = s.h;
@@ -1140,17 +1175,24 @@ static int solve_restarts(const kao_problem *pb, const kao_options *opt, const s
     return KAO_OK;
 }
 
-static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result *res)
+static int solve_impl(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, kao_result *res)
 {
     if (!pb || !opt || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
     int rc = check_search_args(nullptr, opt->rounds, opt->round_size, false);
     if (rc != KAO_OK) return rc;
-    // more than kSmemRowsMax partitions: the large path, which searches with delta evaluation (kao_solve returns the
-    // assignment, whatever evaluator found it) on one GPU per search; refused before anything is searched
-    const bool large = pb->P > kSmemRowsMax;
+    if (tp) {
+        // the topic rows are checked before any CUDA call (each session builds them again)
+        HostModel m;
+        HostTopics ht;
+        std::string why;
+        if (!build_host_model(*pb, m, why) || !build_host_topics(*pb, *tp, m.Ppad, ht, why)) return fail(KAO_E_ARG, why);
+    }
+    // more than kSmemRowsMax partitions, or topic rows: the large path, which searches with delta evaluation (kao_solve
+    // returns the assignment, whatever evaluator found it) on one GPU per search; refused before anything is searched
+    const bool large = pb->P > kSmemRowsMax || tp;
     const bool sharded = (opt->n_gpus > 1 || __builtin_popcount(opt->device_mask) > 1) && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS);
-    if (large && (opt->flags & KAO_FLAG_ROW_MAJOR)) return refuse_large("KAO_FLAG_ROW_MAJOR");
-    if (large && sharded) return refuse_large("n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS (every round sharded over the GPUs)");
+    if (large && (opt->flags & KAO_FLAG_ROW_MAJOR)) return refuse_large("KAO_FLAG_ROW_MAJOR", tp);
+    if (large && sharded) return refuse_large("n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS (every round sharded over the GPUs)", tp);
     if ((opt->flags & KAO_FLAG_LP_BOUND) && !lp_bound_fits(*pb)) return fail(KAO_E_ARG, std::string("KAO_FLAG_LP_BOUND: ") + kLpLimit);
     const auto t0 = std::chrono::steady_clock::now();
     std::vector<int> devs;
@@ -1163,7 +1205,7 @@ static int solve_impl(const kao_problem *pb, const kao_options *opt, kao_result 
     const bool delta = (opt->flags & KAO_FLAG_DELTA) != 0 || large;
     Solved s;
     rc = world > 1 && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS) ? solve_gang(pb, opt, devs, restarts, delta, s)
-                                                                : solve_restarts(pb, opt, devs, restarts, delta, t0, s);
+                                                                : solve_restarts(pb, tp, opt, devs, restarts, delta, t0, s);
     if (rc != KAO_OK) return rc;
     stamp(t0, "session destroyed");
     std::memcpy(res->replicas, s.win.reps.data(), s.win.reps.size() * 4);
@@ -1244,6 +1286,10 @@ extern "C" int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int3
     });
 }
 extern "C" int kao_create(const kao_problem *pb, int32_t device, kao_handle **out) { return guarded([&] { return create_handle(pb, device, out); }); }
+extern "C" int kao_create_topics(const kao_problem *pb, const kao_topics *tp, int32_t device, kao_handle **out)
+{
+    return guarded([&] { return create_handle(pb, device, out, tp); });
+}
 extern "C" int kao_destroy(kao_handle *h) { return guarded([&] { return destroy_impl(h); }); }
 extern "C" int kao_reset(kao_handle *h) { return guarded([&] { return reset_impl(h); }); }
 extern "C" int kao_set_base(kao_handle *h, const int32_t *replicas) { return guarded([&] { return set_base_impl(h, replicas); }); }
@@ -1256,7 +1302,7 @@ extern "C" int kao_round_launch(kao_handle *h, uint64_t seed, uint32_t round, ui
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
-        if (h->large) return refuse_large("kao_round_launch");
+        if (h->large) return refuse_large("kao_round_launch", h->topics);
         if (!check_round_args(round_size) || idx_lo > idx_hi || idx_hi > round_size)
             return fail(KAO_E_ARG, "bad round_size / index range");
         CUDA_TRY(cudaSetDevice(h->device));
@@ -1270,7 +1316,7 @@ extern "C" int kao_round_apply(kao_handle *h, uint64_t seed, uint32_t round, uin
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
-        if (h->large) return refuse_large("kao_round_apply");
+        if (h->large) return refuse_large("kao_round_apply", h->topics);
         if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
         CUDA_TRY(cudaSetDevice(h->device));
         CUDA_TRY(launch_apply(h, seed, round, round_size, reinterpret_cast<const unsigned long long *>(d_key), 0,
@@ -1282,7 +1328,7 @@ extern "C" int kao_set_evaluator(kao_handle *h, int32_t evaluator)
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
-        if (h->large) return refuse_large("kao_set_evaluator");
+        if (h->large) return refuse_large("kao_set_evaluator", h->topics);
         if (evaluator != KAO_EVAL_ROW_MAJOR && evaluator != KAO_EVAL_COLUMN_MAJOR) return fail(KAO_E_ARG, "unknown evaluator");
         if (evaluator == KAO_EVAL_COLUMN_MAJOR && !h->trans_ok)
             return fail(KAO_E_ARG, "column-major evaluator: needs rows of up to 64 slots, racks of up to 8 brokers, at most one "
@@ -1295,7 +1341,7 @@ extern "C" int kao_set_schedule(kao_handle *h, int32_t sync, int32_t pop, int32_
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
-        if (h->large) return refuse_large("kao_set_schedule");
+        if (h->large) return refuse_large("kao_set_schedule", h->topics);
         if (!schedule_exists(sync, pop, threads)) return fail(KAO_E_ARG, "no such schedule (kao.h, kao_set_schedule)");
         h->sch_sync = sync; h->sch_pop = pop; h->sch_threads = threads;
         return KAO_OK;
@@ -1381,5 +1427,9 @@ extern "C" int kao_eval(const kao_problem *pb, int32_t device, const int32_t *re
 }
 extern "C" int kao_solve(const kao_problem *pb, const kao_options *opt, kao_result *res)
 {
-    return guarded([&] { return solve_impl(pb, opt, res); });
+    return guarded([&] { return solve_impl(pb, nullptr, opt, res); });
+}
+extern "C" int kao_solve_topics(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, kao_result *res)
+{
+    return guarded([&] { return solve_impl(pb, tp, opt, res); });
 }

@@ -401,6 +401,42 @@ inline int64_t objective_upper_bound(const HostModel &m, const kao_problem &)
     return total;
 }
 
+// The per-topic rows of a kao_topics (docs/MODEL.md §10), checked against the problem (P, RF): 1 <= T <= P, topic_of
+// in range, 0 <= lo <= hi, and lo no more than the topic can reach.  topic_of as u16 (T <= P <= 65,280), bounds as
+// (C3t lo, C3t hi, C4t lo, C4t hi) per topic.
+struct HostTopics {
+    int T = 0;
+    std::vector<uint16_t> topic_of;           // [Ppad]
+    std::vector<int32_t> bnd;                 // [T][4]
+};
+
+inline bool build_host_topics(const kao_problem &pb, const kao_topics &tp, int Ppad, HostTopics &ht, std::string &why)
+{
+    auto bad = [&](const std::string &s) { why = "topic rows: " + s; return false; };
+    if (tp.T < 1 || tp.T > pb.P) return bad("T must be 1..P");
+    if (!tp.topic_of || !tp.rep_lo || !tp.rep_hi || !tp.ldr_lo || !tp.ldr_hi) return bad("null table pointer");
+    std::vector<int64_t> n(tp.T, 0);
+    ht.T = tp.T;
+    ht.topic_of.assign((size_t)Ppad, 0);
+    for (int p = 0; p < pb.P; ++p) {
+        const int t = tp.topic_of[p];
+        if (t < 0 || t >= tp.T) return bad("topic_of[" + std::to_string(p) + "] = " + std::to_string(t) + " is not in 0..T-1");
+        ht.topic_of[p] = (uint16_t)t;
+        ++n[t];
+    }
+    ht.bnd.assign((size_t)tp.T * 4, 0);
+    for (int t = 0; t < tp.T; ++t) {
+        const int32_t rl = tp.rep_lo[t], rh = tp.rep_hi[t], ll = tp.ldr_lo[t], lh = tp.ldr_hi[t];
+        if (rl < 0 || rl > rh || ll < 0 || ll > lh)
+            return bad("topic " + std::to_string(t) + ": bounds must satisfy 0 <= lo <= hi");
+        if (rl > n[t] * pb.RF || ll > n[t])
+            return bad("topic " + std::to_string(t) + ": lo exceeds what its " + std::to_string(n[t]) +
+                       " partitions can reach (replicas: partitions * RF, leaders: partitions)");
+        ht.bnd[4 * t] = rl; ht.bnd[4 * t + 1] = rh; ht.bnd[4 * t + 2] = ll; ht.bnd[4 * t + 3] = lh;
+    }
+    return true;
+}
+
 inline void fill_consts(const HostModel &m, Consts &cs)
 {
     for (int s = 0; s < 256; ++s) {

@@ -107,6 +107,76 @@ __device__ __forceinline__ void displaced(uint32_t h4, const uint32_t (&row)[W],
     }
 }
 
+__device__ __forceinline__ int band_int(int c, int lo, int hi) { return max(c - hi, 0) + max(lo - c, 0); }
+
+// The topic events of a candidate (docs/MODEL.md §10): a patched row differs from the base by at most one replica
+// move and one leader change, so it gives at most one -1 / +1 replica event and one -1 / +1 valid-leader event, each on
+// the cell topic * 32 W + slot.  Padding slots carry no topic row: -1 (no event) there.
+// Events of patched row i (partition p, leader ldo -> ldn, words old_word(w) -> new_word(w)) into entries 2 i, 2 i + 1.
+template <int W, class Old, class New>
+__device__ __forceinline__ void topic_row_events(const TopicArgs &ta, const Consts *cs, int i, int p, int ldo, int ldn,
+                                                 Old old_word, New new_word, int (&rc)[2 * kMaxOps],
+                                                 int (&lc)[2 * kMaxOps])
+{
+    constexpr int NSL = 32 * W;
+    auto cell = [&](int t, int s) { return (s >= 0 && cs->order_of_slot[s] != 0xFF) ? t * NSL + s : -1; };
+    const int t = ta.topic_of[p];
+    // one word at a time (no row copies: the W = 8 kernel has no registers to spare)
+    int rs = -1, as = -1;
+    bool oko = false, okn = false;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+        const uint32_t o = old_word(w), n = new_word(w);
+        if (o & ~n) rs = 32 * w + __ffs(o & ~n) - 1;
+        if (n & ~o) as = 32 * w + __ffs(n & ~o) - 1;
+        if ((ldo >> 5) == w) oko = (o >> (ldo & 31)) & 1u;
+        if ((ldn >> 5) == w) okn = (n >> (ldn & 31)) & 1u;
+    }
+    rc[2 * i] = cell(t, rs);
+    rc[2 * i + 1] = cell(t, as);
+    lc[2 * i] = cell(t, oko ? ldo : -1);
+    lc[2 * i + 1] = cell(t, okn ? ldn : -1);
+}
+
+// the events of a candidate against the base: entry 2 i is row i's -1 event, 2 i + 1 its +1 event (-1: none)
+template <int W>
+__device__ __forceinline__ void topic_events(const Params &d, const TopicArgs &ta, const Consts *cs, const PatchSet &ps,
+                                             const uint32_t (&rows)[kMaxOps][W], int (&rc)[2 * kMaxOps],
+                                             int (&lc)[2 * kMaxOps])
+{
+#pragma unroll
+    for (int i = 0; i < kMaxOps; ++i) {
+        rc[2 * i] = rc[2 * i + 1] = lc[2 * i] = lc[2 * i + 1] = -1;
+        if (i < ps.n) {
+            const int p = ps.p[i];
+            topic_row_events<W>(ta, cs, i, p, d.leader[p], (int)ps.ld[i],
+                                [&](int w) { return d.bitsT[(size_t)w * d.Ppad + p]; },
+                                [&](int w) { return rows[i][w]; }, rc, lc);
+        }
+    }
+}
+
+// change of the topic-row violation from the base to the candidate: the events netted per cell, <= 12 counts read
+template <int W>
+__device__ __forceinline__ int topic_delta(const TopicArgs &ta, const int (&rc)[2 * kMaxOps], const int (&lc)[2 * kMaxOps])
+{
+    constexpr int LOG2_NSL = W == 1 ? 5 : W == 2 ? 6 : W == 4 ? 7 : 8;
+    int val[2 * kMaxOps];
+#pragma unroll
+    for (int j = 0; j < 2 * kMaxOps; ++j) val[j] = (j & 1) ? 1 : -1;
+    int dv = apply_events<2 * kMaxOps>(rc, val, [&](int c, int net) {
+        const int4 b = __ldg(ta.bnd + (c >> LOG2_NSL));
+        const int n = ta.tcnt[c];
+        return band_int(n + net, b.x, b.y) - band_int(n, b.x, b.y);
+    });
+    dv += apply_events<2 * kMaxOps>(lc, val, [&](int c, int net) {
+        const int4 b = __ldg(ta.bnd + (c >> LOG2_NSL));
+        const int n = ta.tlcnt[c];
+        return band_int(n + net, b.z, b.w) - band_int(n, b.z, b.w);
+    });
+    return dv;
+}
+
 // List changes of one round: at most kMaxOps removals and insertions per list
 struct ListChanges {
     int nd[2], ni[2];
@@ -222,10 +292,35 @@ __device__ void apply_winner_large(const Params &d, const LargeArgs &la, const C
     }
 }
 
+// CTA 0, the thread that wrote the winner record (apply_winner_large): the topic counts and the topic-row violation of
+// the base follow the record's old and new rows
 template <int W>
+__device__ __forceinline__ void apply_winner_topics(const TopicArgs &ta, const Consts *cs, const LargeRecord &rec)
+{
+    int rc[2 * kMaxOps], lc[2 * kMaxOps];
+#pragma unroll
+    for (int i = 0; i < kMaxOps; ++i) {
+        rc[2 * i] = rc[2 * i + 1] = lc[2 * i] = lc[2 * i + 1] = -1;
+        if (i < rec.n)
+            topic_row_events<W>(ta, cs, i, rec.p[i], (int)rec.old_ld[i], (int)rec.new_ld[i],
+                                [&](int w) { return rec.old_row[i][w]; }, [&](int w) { return rec.new_row[i][w]; },
+                                rc, lc);
+    }
+    *ta.tviol += topic_delta<W>(ta, rc, lc);
+#pragma unroll
+    for (int j = 0; j < 2 * kMaxOps; ++j) {
+        const int v = (j & 1) ? 1 : -1;
+        if (rc[j] >= 0) ta.tcnt[rc[j]] = (uint16_t)(ta.tcnt[rc[j]] + v);
+        if (lc[j] >= 0) ta.tlcnt[lc[j]] = (uint16_t)(ta.tlcnt[lc[j]] + v);
+    }
+}
+
+// the search kernel; kTopics: the topic rows of ta are part of the violation (ta is unused otherwise and comes last,
+// so that the parameters of the plain instantiations are laid out as without it)
+template <int W, bool kTopics>
 __global__ void __launch_bounds__(kLT, 1)
 search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
-                    unsigned long long *keys, unsigned int *grid_bar, P2P pp, unsigned long long *all_keys)
+                    unsigned long long *keys, unsigned int *grid_bar, P2P pp, unsigned long long *all_keys, TopicArgs ta)
 {
     constexpr int kWarps = kLT / 32, NSL = 32 * W;
     __shared__ Consts s_cs;
@@ -253,6 +348,9 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
         // the evaluation IS the previous winner's key (unless that key was saturated)
         if (t == 0 || s_base[2] == 0) {
             block_eval<W>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc);
+            if constexpr (kTopics) {
+                if (tid == 0) s_acc[0] += __ldcg(ta.tviol);
+            }
             if (tid == 0) { s_base[0] = (int)min(s_acc[0], (long long)0x7FFFFFFF); s_base[1] = (int)s_acc[1]; }
             __syncthreads();
         }
@@ -268,6 +366,11 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
                 int viol, obj;
                 delta_eval<LargeCfg<W>, false>(d, d.bitsT, d.leader, m_obj, &s_cs, ps, rows, s_cnt, s_lcnt, s_rc,
                                                base_viol, base_obj, viol, obj);
+                if constexpr (kTopics) {
+                    int rc[2 * kMaxOps], lc[2 * kMaxOps];
+                    topic_events<W>(d, ta, &s_cs, ps, rows, rc, lc);
+                    viol += topic_delta<W>(ta, rc, lc);
+                }
                 const unsigned long long key = pack_key(viol, obj, idx, d.key_obj_bits);
                 if (all_keys) all_keys[idx - pp.idx_lo] = key;
                 best = key < best ? key : best;
@@ -319,6 +422,9 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
             continue;
         }
         if (blockIdx.x == 0) apply_winner_large<W>(d, la, &s_cs, s_st, seed, round, round_size, k, s_rec, s_lc);
+        if constexpr (kTopics) {
+            if (blockIdx.x == 0 && tid == 0) apply_winner_topics<W>(ta, &s_cs, s_rec);
+        }
         // grid barrier 2: the patched HBM state and the winner record are visible before anyone reads them
         __syncthreads();
         if (tid == 0) {
@@ -354,6 +460,51 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
         __syncthreads();
         if (s_red[kWarps]) break;
     }
+}
+
+// a topic session's counts: one 32-bit atomic on the word that holds the u16 cell (a cell never exceeds 65,280)
+template <int W>
+__global__ void topic_count_kernel(Params d, TopicArgs ta)
+{
+    constexpr int NSL = 32 * W;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < d.P; p += gridDim.x * blockDim.x) {
+        const int t = ta.topic_of[p], ld = d.leader[p];
+        uint32_t x[W];
+#pragma unroll
+        for (int w = 0; w < W; ++w) x[w] = d.bitsT[(size_t)w * d.Ppad + p];
+        auto bump = [&](uint16_t *c, int s) {
+            const size_t i = (size_t)t * NSL + s;
+            atomicAdd(reinterpret_cast<unsigned int *>(c + (i & ~(size_t)1)), 1u << (16 * (i & 1)));
+        };
+#pragma unroll
+        for (int w = 0; w < W; ++w)
+            for (uint32_t m = x[w]; m; m &= m - 1) {
+                const int s = 32 * w + __ffs(m) - 1;
+                if (d.consts->order_of_slot[s] != 0xFF) bump(ta.tcnt, s);
+            }
+        if (ld < NSL && row_has<W>(x, ld) && d.consts->order_of_slot[ld] != 0xFF) bump(ta.tlcnt, ld);
+    }
+}
+
+// the topic-row violation of the base: every (topic, broker slot) cell once
+template <int W>
+__global__ void topic_violation_kernel(Params d, TopicArgs ta)
+{
+    constexpr int NSL = 32 * W;
+    __shared__ int s_v;
+    if (threadIdx.x == 0) s_v = 0;
+    __syncthreads();
+    int v = 0;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)ta.T * NSL; i += (size_t)gridDim.x * blockDim.x) {
+        const int s = (int)(i & (NSL - 1));
+        if (d.consts->order_of_slot[s] == 0xFF) continue;
+        const int4 b = ta.bnd[i / NSL];
+        v += band_int(ta.tcnt[i], b.x, b.y) + band_int(ta.tlcnt[i], b.z, b.w);
+    }
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0 && v) atomicAdd(&s_v, v);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_v) atomicAdd(ta.tviol, s_v);
 }
 
 // the transposed planes of the base (every word, the padding words of t_words included)
@@ -401,6 +552,20 @@ eval_large_kernel(Params d, const uint32_t *bits, const uint8_t *leader, long lo
     if (threadIdx.x == 0) { viol[a] = s_acc[0]; obj[a] = s_acc[1]; }
 }
 
+// a topic session's base: the evaluation above plus the topic-row violation kept current with the base
+template <int W>
+__global__ void __launch_bounds__(kLT, 1)
+eval_large_topics_kernel(Params d, TopicArgs ta, long long *viol, long long *obj)
+{
+    __shared__ Consts s_cs;
+    __shared__ int s_cnt[256], s_lcnt[256], s_rc[32];
+    __shared__ long long s_acc[2];
+    load_consts(&s_cs, d.consts);
+    __syncthreads();
+    block_eval<W>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc);
+    if (threadIdx.x == 0) { *viol = s_acc[0] + __ldcg(ta.tviol); *obj = s_acc[1]; }
+}
+
 template <class F> cudaError_t with_w(int W, F &&f)
 {
     switch (W) {
@@ -423,18 +588,45 @@ cudaError_t large_prepare(int W, const Params &d, const LargeArgs &la, cudaStrea
     });
 }
 
+cudaError_t topics_prepare(int W, const Params &d, const TopicArgs &ta, cudaStream_t st)
+{
+    const size_t cells = (size_t)ta.T * 32 * W;
+    cudaError_t e = cudaMemsetAsync(ta.tcnt, 0, cells * 2, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ta.tlcnt, 0, cells * 2, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ta.tviol, 0, sizeof(int), st);
+    if (e != cudaSuccess) return e;
+    return with_w(W, [&](auto w) {
+        constexpr int kW = decltype(w)::value;
+        topic_count_kernel<kW><<<264, 256, 0, st>>>(d, ta);
+        topic_violation_kernel<kW><<<528, 256, 0, st>>>(d, ta);
+        return cudaGetLastError();
+    });
+}
+
 cudaError_t large_search(int W, int grid, const Params &d, const LargeArgs &la, uint64_t seed, uint32_t first_round,
                          uint32_t rounds, uint32_t round_size, unsigned long long *keys, unsigned int *grid_bar,
-                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st)
+                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st, const TopicArgs *ta)
 {
     Params prm = d;
     LargeArgs a = la;
     P2P p2 = pp;
-    void *args[] = {&prm, &a, &seed, &first_round, &rounds, &round_size, &keys, &grid_bar, &p2, &all_keys};
+    TopicArgs t = ta ? *ta : TopicArgs{};
+    void *args[] = {&prm, &a, &seed, &first_round, &rounds, &round_size, &keys, &grid_bar, &p2, &all_keys, &t};
     return with_w(W, [&](auto w) {
+        constexpr int kW = decltype(w)::value;
         // cooperative launch: all CTAs are co-resident, which the grid barriers need
-        return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(search_large_kernel<decltype(w)::value>),
-                                           dim3(grid), dim3(kLT), args, 0, st);
+        const void *kern = ta ? reinterpret_cast<const void *>(search_large_kernel<kW, true>)
+                              : reinterpret_cast<const void *>(search_large_kernel<kW, false>);
+        return cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kLT), args, 0, st);
+    });
+}
+
+cudaError_t large_eval_topics(int W, const Params &d, const TopicArgs &ta, long long *viol, long long *obj,
+                              cudaStream_t st)
+{
+    return with_w(W, [&](auto w) {
+        eval_large_topics_kernel<decltype(w)::value><<<1, kLT, 0, st>>>(d, ta, viol, obj);
+        return cudaGetLastError();
     });
 }
 

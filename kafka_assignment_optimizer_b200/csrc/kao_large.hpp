@@ -32,15 +32,31 @@ struct LargeArgs {
     LargeRecord *rec;
 };
 
+// Per-topic balance rows of a topic session (docs/MODEL.md §10, DESIGN.md §7.2), all in HBM.  The counts are those of
+// the base over broker slots (padding slots are never counted nor read); CTA 0 patches them and tviol from each
+// round's winner before the second grid barrier.
+struct TopicArgs {
+    int T;
+    const uint16_t *topic_of;       // [Ppad] topic of each partition
+    const int4 *bnd;                // [T] (C3t lo, C3t hi, C4t lo, C4t hi)
+    uint16_t *tcnt, *tlcnt;         // [T][32 W] replicas / valid leaders of each topic per slot
+    int *tviol;                     // the base's violation of the topic rows
+};
+
 // the HBM state derived from the base (transposed planes, displaced lists in buffer 0, leader validity count) after
 // the base itself was uploaded
 cudaError_t large_prepare(int W, const Params &d, const LargeArgs &la, cudaStream_t st);
+// a topic session's counts and topic-row violation of the base, from scratch
+cudaError_t topics_prepare(int W, const Params &d, const TopicArgs &ta, cudaStream_t st);
 // rounds first_round .. first_round + rounds - 1 of a delta search in one cooperative launch (one CTA per SM);
 // P2P: rank 0 of 1 (idx_lo / idx_hi, early stop, abort flag, rounds run).  all_keys != nullptr: one round, every
-// candidate's key dumped, the base left as it is
+// candidate's key dumped, the base left as it is.  ta != nullptr: with the topic rows
 cudaError_t large_search(int W, int grid, const Params &d, const LargeArgs &la, uint64_t seed, uint32_t first_round,
                          uint32_t rounds, uint32_t round_size, unsigned long long *keys, unsigned int *grid_bar,
-                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st);
+                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st, const TopicArgs *ta = nullptr);
 // full evaluation of n explicit assignments (bits [n][W][Ppad], leaders [n][Ppad]): one CTA each
 cudaError_t large_eval(int W, const Params &d, const uint32_t *bits, const uint8_t *leader, int n, long long *viol,
                        long long *obj, cudaStream_t st);
+// full evaluation of a topic session's base, topic rows included
+cudaError_t large_eval_topics(int W, const Params &d, const TopicArgs &ta, long long *viol, long long *obj,
+                              cudaStream_t st);

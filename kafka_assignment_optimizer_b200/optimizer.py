@@ -10,8 +10,8 @@ from typing import Optional
 
 import numpy as np
 
-from .problem import (Problem, build_problem, parse_assignment_json, parse_broker_list, parse_rack_map,
-                      reassignment_json)
+from .problem import (Problem, TopicRows, build_problem, parse_assignment_json, parse_broker_list, parse_rack_map,
+                      reassignment_json, topic_rows)
 
 _LIB_PATH = os.environ.get("KAO_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libkao.so")
 KAO_OK, KAO_INFEASIBLE = 0, 1
@@ -135,6 +135,25 @@ class _CProblem:
         return C.byref(self.c)
 
 
+class _KaoTopics(C.Structure):
+    _fields_ = [("T", C.c_int32), ("topic_of", C.c_void_p), ("rep_lo", C.c_void_p), ("rep_hi", C.c_void_p),
+                ("ldr_lo", C.c_void_p), ("ldr_hi", C.c_void_p)]
+
+
+class _CTopics:
+    """kao_topics over contiguous copies of a TopicRows (None: no topic rows, a NULL pointer)."""
+
+    def __init__(self, tr: Optional[TopicRows]):
+        self.c = None
+        if tr is not None:
+            self.keep = [np.ascontiguousarray(x, dtype=np.int32) for x in
+                         (tr.topic_of, tr.rep_lo, tr.rep_hi, tr.ldr_lo, tr.ldr_hi)]
+            self.c = _KaoTopics(len(self.keep[1]), *(x.ctypes.data for x in self.keep))
+
+    def ref(self):
+        return None if self.c is None else C.byref(self.c)
+
+
 @dataclasses.dataclass
 class SolveResult:
     replicas: np.ndarray      # int32 [P, RF] dense broker indices, leader first
@@ -154,14 +173,19 @@ class SolveResult:
 
 
 class Session:
-    """Device-resident problem (kao_create .. kao_destroy)."""
+    """Device-resident problem (kao_create .. kao_destroy).  topics: per-topic balance rows (a TopicRows, e.g.
+    topic_rows(pb)) through kao_create_topics; such a session searches with delta evaluation only."""
 
-    def __init__(self, pb: Problem, device: int = 0):
+    def __init__(self, pb: Problem, device: int = 0, topics: Optional[TopicRows] = None):
         self.pb = pb
         self._cp = _CProblem(pb)
         self._h = C.c_void_p()
         self._lib = load_library()
-        _check(self._lib.kao_create(self._cp.ref(), C.c_int32(device), C.byref(self._h)))
+        if topics is None:
+            _check(self._lib.kao_create(self._cp.ref(), C.c_int32(device), C.byref(self._h)))
+        else:
+            self._ct = _CTopics(topics)
+            _check(self._lib.kao_create_topics(self._cp.ref(), self._ct.ref(), C.c_int32(device), C.byref(self._h)))
         self.key_obj_bits = self._lib.kao_key_obj_bits(self._cp.ref())
 
     def unpack_key(self, key):
@@ -314,21 +338,31 @@ class Session:
 def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 1 << 15,
           device: int = 0, require_feasible: bool = False, restarts: int = 1, delta: bool = False,
           patience: int = 0, row_major: bool = False, n_gpus: int = 1, device_mask: int = 0,
-          tight_bound: bool = False, spread_restarts: bool = False, lp_bound: bool = False) -> SolveResult:
+          tight_bound: bool = False, spread_restarts: bool = False, lp_bound: bool = False,
+          topic_balance: bool = False, topics: Optional[TopicRows] = None) -> SolveResult:
     """One blocking kao_solve from host buffers (tables up, winner down).  n_gpus > 1: every round is sharded
     over that many GPUs of this process (devices device .. device+n_gpus-1, or those of device_mask), or with
     spread_restarts the restarts run side by side, one single-GPU search per GPU at a time; either way the
     result is the same as on one GPU with the same arguments.  tight_bound / lp_bound: objective_bound from the flow
-    bound (KAO_FLAG_BOUND) / also from the Lagrangian LP bound (KAO_FLAG_LP_BOUND); either can prove optimality."""
+    bound (KAO_FLAG_BOUND) / also from the Lagrangian LP bound (KAO_FLAG_LP_BOUND); either can prove optimality.
+    topic_balance: every topic spread over the brokers too (kao_solve_topics with `topics`, by default
+    topic_rows(pb)); the bounds then leave the topic rows out and may be looser."""
     lib = load_library()
     cp = _CProblem(pb)
+    if topic_balance and topics is None:
+        topics = topic_rows(pb)
     reps = np.full((pb.P, pb.RF), -1, np.int32)
     flags = (max(1, min(255, restarts)) | (0x100 if delta else 0) | (0x200 if row_major else 0) | (0x400 if tight_bound else 0) | (0x800 if spread_restarts else 0) | (0x1000 if lp_bound else 0) |
              (max(0, min(65535, patience)) << 16))
     opt = _KaoOptions(seed & (2 ** 64 - 1), rounds, round_size, device, flags, n_gpus, device_mask)
     res = _KaoResult()
     res.replicas = reps.ctypes.data
-    rc = _check(lib.kao_solve(cp.ref(), C.byref(opt), C.byref(res)), allow_infeasible=not require_feasible)
+    if topics is None:
+        rc = _check(lib.kao_solve(cp.ref(), C.byref(opt), C.byref(res)), allow_infeasible=not require_feasible)
+    else:
+        ct = _CTopics(topics)
+        rc = _check(lib.kao_solve_topics(cp.ref(), ct.ref(), C.byref(opt), C.byref(res)),
+                    allow_infeasible=not require_feasible)
     return SolveResult(reps, res.objective, res.violation, res.moves, rc == KAO_OK, res.key,
                        res.n_candidates, res.rounds_run, res.device_ms, res.total_ms, res.objective_bound,
                        bool(res.optimal), res.key_obj_bits, res.n_gpus)

@@ -102,6 +102,41 @@ def synthetic_problem(P: int, B0: int, R: int, RF: int, remove: int = 0, perturb
     return build_problem(current, range(B0 - remove), {b: "r%02d" % (b % R) for b in range(B0)}, RF)
 
 
+@dataclasses.dataclass
+class TopicRows:
+    """Per-topic balance rows (kao_topics, docs/MODEL.md §10): for every topic t and broker, the replicas of t's
+    partitions there within [rep_lo[t], rep_hi[t]] (C3t) and the partitions of t led from there within
+    [ldr_lo[t], ldr_hi[t]] (C4t)."""
+    topic_of: np.ndarray    # int32 [P]  topic index of each row
+    rep_lo: np.ndarray      # int32 [T]
+    rep_hi: np.ndarray
+    ldr_lo: np.ndarray      # int32 [T]
+    ldr_hi: np.ndarray
+    names: list             # [T] topic names
+
+    @property
+    def T(self) -> int:
+        return len(self.names)
+
+
+def topic_rows(pb: Problem) -> TopicRows:
+    """The default per-topic rows of `pb`: the topics of pb.topics (one topic "t1" for all rows when absent) in order of
+    first appearance, bounds floor / ceil of n_t * RF / B for replicas and of n_t / B for leaders (n_t = the topic's
+    partitions), the §1 formulas of C3 / C4 per topic.  For the README's one topic they are its rows C3 / C4
+    (README.md:158-166)."""
+    names, index = [], {}
+    topic_of = np.zeros(pb.P, np.int32)
+    for p in range(pb.P):
+        name = pb.topics[p][0] if pb.topics else "t1"
+        if name not in index:
+            index[name] = len(names)
+            names.append(name)
+        topic_of[p] = index[name]
+    n = np.bincount(topic_of, minlength=len(names)).astype(np.int64)
+    return TopicRows(topic_of, (n * pb.RF // pb.B).astype(np.int32), (-(-n * pb.RF // pb.B)).astype(np.int32),
+                     (n // pb.B).astype(np.int32), (-(-n // pb.B)).astype(np.int32), names)
+
+
 # ---------------------------------------------------------------------------------- Kafka JSON
 def parse_assignment_json(text: str):
     """`kafka-reassign-partitions --generate` "Current partition replica assignment" JSON

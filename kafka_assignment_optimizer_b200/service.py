@@ -8,7 +8,7 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
                    "racks": "0:a,1:b,...",                               README.md:27-29
                    "rf": 2, "rounds": 256, "round_size": 32768, "restarts": 1, "patience": 0, "delta": false,
                    "gpus": 1, "spread_restarts": false, "certificate": false,
-                   "lp_certificate": false}
+                   "lp_certificate": false, "topic_balance": false}
     200           {"reassignment": {"version":1,"partitions":[...]},    README.md:67-78
                    "objective": ..., "violation": ..., "moves": ..., "feasible": ...,
                    "objective_bound": ..., "proven_optimal": ...}
@@ -16,7 +16,8 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
 `gpus` > 1 shards every round over that many GPUs (or, with `spread_restarts`, runs the restarts side by side);
 `certificate` asks for the flow bound, so that `proven_optimal` can say the answer is what lp_solve would return
 (README.md:135-136); `lp_certificate` also asks for the Lagrangian LP bound (GPU, docs/MODEL.md §9), which proves
-optima the flow bound cannot, e.g. after brokers are removed.
+optima the flow bound cannot, e.g. after brokers are removed.  `topic_balance` also spreads every topic over the
+brokers (the per-topic rows of docs/MODEL.md §10, default bounds of `topic_rows`).
 
 `python -m kafka_assignment_optimizer_b200.service --port 8080` (needs a GPU: there is no CPU path).
 """
@@ -61,10 +62,12 @@ def handle_submit(body: dict, solver: Optional[Callable] = None) -> dict:
     if rounds * round_size * restarts > MAX_CANDIDATES:
         raise ValueError("rounds * round_size * restarts exceeds %d candidates per request" % MAX_CANDIDATES)
     gpus = _bounded(body, "gpus", 1, 1, 8)                      # KAO_MAX_GPUS
+    # only asked for when wanted: a solver without topic rows keeps its signature
+    extra = {"topic_balance": True} if body.get("topic_balance") else {}
     res = solver(pb, seed=int(body.get("seed", 0x5EED)) & (2**64 - 1), rounds=rounds, round_size=round_size,
                  restarts=restarts, delta=bool(body.get("delta", False)), patience=patience, n_gpus=gpus,
                  spread_restarts=bool(body.get("spread_restarts", False)), tight_bound=bool(body.get("certificate", False)),
-                 lp_bound=bool(body.get("lp_certificate", False)))
+                 lp_bound=bool(body.get("lp_certificate", False)), **extra)
     return {"reassignment": reassignment_json(pb, res.replicas), "objective": int(res.objective),
             "violation": int(res.violation), "moves": int(res.moves), "feasible": bool(res.feasible),
             "objective_bound": int(res.objective_bound), "proven_optimal": bool(res.optimal)}
