@@ -129,6 +129,38 @@ __device__ __forceinline__ int reduce_scatter8(int (&v)[8], int lane)
 }
 
 // ------------------------------------------------------------------------------------------
+// Sorted batches (schedules with pop digit 2 = 3).  The 32 lanes of a batch run the union of their candidates'
+// generator bodies, and every branch of that union is chosen by the candidate's control word (docs/MODEL.md §5),
+// which depends on (seed, round, index) alone, not on the base.  So a CTA sorts its candidates of a round by the
+// class below before the round starts, and a batch takes 32 neighbours of that order: mostly one body.  The class:
+// 0 the identity candidate; in a cycle round 1 + the two role-match bits (every other choice is fixed there); else
+// operations << 6 | first-operation LEADER << 5 | guided << 4 | link kind of operation 2 << 2 | of operation 3
+// (link kinds of operations a candidate does not have are 0).  Below kCandClasses (kao_plan.hpp).
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cand_class(uint64_t seed, uint32_t round, uint32_t idx, uint32_t round_size)
+{
+    if (idx + 1 == round_size) return 0;
+    uint32_t r[4];
+    philox4x32_10(idx, round, 0u, kTag, (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    const uint32_t ctl = r[0];
+    if ((round & 3u) == 3u) return 1u + ((ctl >> 11) & 1u) * 2u + ((ctl >> 13) & 1u);
+    const uint32_t nops = (ctl & 3u) == 0 ? 1u : ((ctl & 3u) == 3 ? 3u : 2u);
+    return nops << 6 | ((ctl >> 2) & 3u) << 4 | (nops >= 2 ? ((ctl >> 4) & 3u) << 2 : 0u) | (nops == 3 ? (ctl >> 7) & 3u : 0u);
+}
+// candidate index at position k of a CTA's share of a round: warp k % warps, iteration k / warps
+__host__ __device__ __forceinline__ uint32_t cand_at(uint32_t k, uint32_t first, uint32_t stride, uint32_t warps)
+{
+    return first + k % warps + k / warps * stride;
+}
+// how many of the positions 0, 1, ... of a CTA's share lie below idx_hi (indices rise with the position)
+__host__ __device__ __forceinline__ uint32_t cand_count(uint32_t first, uint32_t stride, uint32_t warps, uint32_t idx_hi)
+{
+    if (first >= idx_hi) return 0;
+    const uint32_t full = (idx_hi - first) / stride, rem = (idx_hi - first) % stride;
+    return full * warps + (rem < warps ? rem : warps);
+}
+
+// ------------------------------------------------------------------------------------------
 // The batch of 32 candidates.  T: the transposed planes; Z: term, rack-field and shortfall planes ([kZPlanes + 4 W +
 // kSPlanes][nW]); batch: the warp's parked candidates.  Returns, in lane (g, t), candidate mma_lane_candidate(lane):
 // its violation and objective.

@@ -281,8 +281,11 @@ template <bool kDelta> struct LaunchPersistent {
         cudaError_t e = set_smem_attr(h, reinterpret_cast<const void *>(kern), done);
         if (e != cudaSuccess) return e;
         Params prm = h->prm;
-        // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch)
-        SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF, cfg_mma<Cfg>())
+        // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch) and, with sorted batches,
+        // on the candidates of a CTA per round (the most any CTA takes: its warps' iterations)
+        const uint32_t stride = (uint32_t)h->grid * (T / 32), share = a.pp.idx_hi - a.pp.idx_lo;
+        const uint32_t cands = cfg_sorted<Cfg>() ? (share + stride - 1) / stride * (T / 32) : 0;
+        SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF, cfg_mma<Cfg>(), cands)
                         : (kDelta && Cfg::W > 2) ? make_plan_delta_wide(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF) : h->plan;
         if (plan.total > 227u * 1024u) return cudaErrorInvalidConfiguration;
         uint64_t seed = a.seed; uint32_t fr = a.first_round, rounds = a.rounds, rs = a.round_size;

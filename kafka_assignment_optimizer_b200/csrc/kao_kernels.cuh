@@ -34,6 +34,12 @@ template <class Cfg> __host__ __device__ constexpr bool cfg_mma()
     if constexpr (Cfg::kTrans) return Cfg::kSums >= 1;
     else return false;
 }
+// does a configuration take its batches from the CTA's candidates sorted by class (kao_device_mma.cuh, cand_class)
+template <class Cfg> __host__ __device__ constexpr bool cfg_sorted()
+{
+    if constexpr (Cfg::kTrans) return Cfg::kSums == 3;
+    else return false;
+}
 
 // ------------------------------------------------------------------------------------------
 // PTX wrappers: mbarrier + TMA bulk copy (SASS: SYNCS / UBLKCP)
@@ -67,8 +73,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
 // warp.  Without the flag KAO_PHASE(...) expands to nothing: the shipped kernels are compiled from the same tokens.
 #if defined(KAO_PHASE_CLOCKS)
 // per (CTA, warp, round): summed cycles of generate + park and of eval_batch_mma, the batches, and the stamps at the
-// round's start, after the warp's last batch, after the CTA reduce, the grid barrier, the winner's patch and rebuild_lists
-enum PhaseSlot { kPhGen, kPhEval, kPhBatches, kPhStart, kPhBatchesEnd, kPhReduce, kPhBarrier, kPhApply, kPhRebuild, kPhSlots };
+// round's start, after the warp's last batch, after the CTA reduce, the grid barrier, the winner's patch and rebuild_lists;
+// warps 1 .. of a sorted-batch schedule: after they sorted the next round's candidates (in the grid barrier's time)
+enum PhaseSlot { kPhGen, kPhEval, kPhBatches, kPhStart, kPhBatchesEnd, kPhReduce, kPhBarrier, kPhApply, kPhRebuild, kPhList, kPhSlots };
 constexpr int kPhaseWarps = 32, kPhaseRounds = 64;
 static __device__ unsigned long long *kao_phase_buf;
 __device__ __forceinline__ unsigned long long *phase_rec(int warp, uint32_t t)
@@ -396,6 +403,46 @@ __device__ __forceinline__ void bind_tables(Gen<W, true, kSmall> &tg, const Roun
     tg.inv_ok = *rt.inv != 0; tg.hoff = rt.hoff; tg.loff = rt.loff; tg.hold = rt.hold; tg.led = rt.led;
 }
 
+// Sorted batches: the n candidates of a CTA's share of a round (cand_at) as a list sorted by cand_class, by counting
+// sort — histogram, exclusive scan, scatter.  Built by the NT threads t = 0 .. NT - 1 of warps kWarps - NT / 32 ..
+// kWarps - 1, which meet at named barrier 1 (or by the whole CTA: __syncthreads).  The order within a class is
+// arbitrary (shared-memory atomics): a key carries its candidate's index, so neither the minima nor all_keys depend
+// on which lane evaluates which candidate.
+template <int kWarps, int NT>
+__device__ __noinline__ void build_cand_list(uint32_t *list, uint8_t *cls, int *hist, uint32_t n, uint32_t first, uint32_t stride,
+                                             uint64_t seed, uint32_t round, uint32_t round_size, int t)
+{
+    static_assert(NT % 32 == 0 && NT <= kWarps * 32 && kCandClasses == 256, "whole warps; 8 classes per lane of the scan");
+    auto sync = [] {
+        if constexpr (NT == kWarps * 32) __syncthreads();
+        else asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
+    };
+    for (int c = t; c < (int)kCandClasses; c += NT) hist[c] = 0;
+    sync();
+    for (uint32_t k = t; k < n; k += NT) {
+        const uint32_t c = cand_class(seed, round, cand_at(k, first, stride, kWarps), round_size);
+        cls[k] = (uint8_t)c;
+        atomicAdd(&hist[c], 1);
+    }
+    sync();
+    if (t < 32) {
+        int v[8], s = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { v[i] = hist[8 * t + i]; s += v[i]; }
+        int incl = s;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (t >= o) incl += u;
+        }
+        int run = incl - s;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { hist[8 * t + i] = run; run += v[i]; }
+    }
+    sync();
+    for (uint32_t k = t; k < n; k += NT) list[atomicAdd(&hist[cls[k]], 1)] = cand_at(k, first, stride, kWarps);
+}
+
 // Column-major kernels: the 32 lanes of a warp generate 32 candidates at once (one each, per-thread
 // generator) and park them in the warp's scratch; the warp then evaluates them one after the other.
 // Scratch per candidate: 3 partitions, (leader slots | count << 24), 3 x W row words (16-byte aligned).
@@ -474,6 +521,20 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
     const uint32_t stride = gridDim.x * kWarps;
     const uint32_t first = pp.idx_lo + blockIdx.x * kWarps;
     const uint32_t iters = first < pp.idx_hi ? (pp.idx_hi - first + stride - 1) / stride : 0;
+    // sorted batches: the CTA's candidates of a round sorted by class, behind the class histogram.  A share beyond the
+    // plan's list (rounds near KAO_MAX_ROUND_SIZE) walks its candidates unsorted, as the other schedules do
+    constexpr bool kSorted = cfg_sorted<Cfg>();
+    int *s_hist = reinterpret_cast<int *>(smem + plan.off_inv);
+    uint32_t *s_list = reinterpret_cast<uint32_t *>(s_hist + kCandClasses);
+    uint8_t *s_cls = reinterpret_cast<uint8_t *>(s_list + cand_list_cap(plan));
+    const uint32_t n_cta = kSorted ? cand_count(first, stride, kWarps, pp.idx_hi) : 0u;
+    const bool sorted = kSorted && n_cta <= cand_list_cap(plan);
+    if constexpr (kSorted) {
+        if (sorted && rounds > 0) {                             // round 0's list; each later one during the round before
+            build_cand_list<kWarps, THREADS>(s_list, s_cls, s_hist, n_cta, first, stride, seed, first_round, round_size, tid);
+            __syncthreads();
+        }
+    }
     if (tid == 0) s_abort = 0;
     // early-stop state lives behind the per-warp minima (s_red is live anyway; a separate pointer would
     // cost a register in the hot loop): [kWarps] stop flag, [kWarps+1] best (violation, cost), [kWarps+2] stall
@@ -529,19 +590,29 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
             // ---- column-major evaluator, sums on the tensor cores (kao_device_mma.cuh): candidates are generated 32 at a
             // time, one per LANE, as below, then the warp evaluates all 32 together; lane (g, t) ends with the
             // violation and objective of candidate mma_lane_candidate(lane) of the batch.  Pop digit 2 = 2: the later
-            // operations' link kinds share their steps (Gen kMerged), same candidates
-            Gen<W, true, true, Cfg::kSums == 2> tg;        // compact code (row_kth keeps its loop), same candidates
+            // operations' link kinds share their steps (Gen kMerged), same candidates.  Pop digit 2 = 3: as 2, and the batches
+            // come from the CTA's candidates sorted by class (s_list), batch b of them to warp b mod kWarps, so that every
+            // warp takes a share of each class
+            Gen<W, true, true, Cfg::kSums >= 2> tg;        // compact code (row_kth keeps its loop), same candidates
             tg.bitsT = s_bits; tg.leader = s_leader; tg.cs = s_cs; tg.d = &d; tg.prow = nullptr; tg.lane = 0;
             tg.D = s_D; tg.DL = s_DL; tg.nD = s_counts[0]; tg.nL = s_counts[1];
             tg.T = s_sw; tg.tnW = t_words(d.Ppad); tg.t_leaders_valid = s_counts[2] == 0;    // "first holder of slot s": plane scan
             uint32_t *batch = s_prow + (size_t)warp * 32 * batch_stride<W>();
             const uint32_t j = (uint32_t)mma_lane_candidate(lane);
-            for (uint32_t it0 = 0; it0 < iters; it0 += 32) {
+            const uint32_t nbatch = sorted ? (n_cta + 31) / 32 : (iters + 31) / 32;
+            for (uint32_t b = sorted ? warp : 0; b < nbatch; b += sorted ? kWarps : 1) {
                 KAO_PHASE(const unsigned long long ph0 = clock64();)
                 mma_clear_batch<W>(batch, lane);
                 __syncwarp();
+                const uint32_t it0 = 32 * b;
+                uint32_t mine = first + warp + (it0 + lane) * stride;
+                bool live = it0 + lane < iters && mine < pp.idx_hi;
+                if (sorted) {
+                    live = it0 + lane < n_cta;
+                    mine = live ? s_list[it0 + lane] : 0u;
+                }
                 {
-                    const uint32_t idx = first + warp + (it0 + lane) * stride;
+                    const uint32_t idx = mine;
                     PatchSet ps;
                     uint32_t rows[kMaxOps][W];
                     ps.n = 0;
@@ -551,7 +622,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 #pragma unroll
                         for (int w = 0; w < W; ++w) rows[i][w] = 0;
                     }
-                    if (it0 + lane < iters && idx < pp.idx_hi) tg.run(seed, round, idx, round_size, ps, rows);
+                    if (live) tg.run(seed, round, idx, round_size, ps, rows);
                     int pviol, pobj, pcount;
                     patch_terms<W>(d, ps, rows, pviol, pobj, pcount);
                     mma_park_patch<W>(ps, rows, pviol, pobj, batch, lane);
@@ -562,8 +633,13 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                 eval_batch_mma<Cfg>(d, s_cs, s_sw, t_words(d.Ppad), s_z, batch, lane, viol, obj);
                 KAO_PHASE(asm volatile("" ::"r"(viol), "r"(obj)); const unsigned long long ph2 = clock64();
                           ph_gen += ph1 - ph0; ph_eval += ph2 - ph1; ++ph_n;)
-                const uint32_t idx = first + warp + (it0 + j) * stride;
-                if (it0 + j < iters && idx < pp.idx_hi) {
+                uint32_t idx = first + warp + (it0 + j) * stride;
+                bool live_j = it0 + j < iters && idx < pp.idx_hi;
+                if (sorted) {                                               // candidate j of the batch was lane j's
+                    idx = __shfl_sync(0xFFFFFFFFu, mine, j);
+                    live_j = it0 + j < n_cta;
+                }
+                if (live_j) {
                     const unsigned long long key = pack_key(viol, obj, idx, d.key_obj_bits);
                     if (all_keys) all_keys[idx - pp.idx_lo] = key;
                     best = key < best ? key : best;                 // equal (violation, cost): the lowest index
@@ -719,6 +795,14 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                 }
             }
         }
+        if constexpr (kSorted) {
+            // the other warps sort the next round's candidates while warp 0 waits at the grid barrier: the classes
+            // depend on (seed, round, index) alone, not on the winner
+            if (warp != 0 && sorted && t + 1 < rounds) {
+                build_cand_list<kWarps, THREADS - 32>(s_list, s_cls, s_hist, n_cta, first, stride, seed, round + 1, round_size, tid - 32);
+                KAO_PHASE(if (ph) ph[kPhList] = clock64();)
+            }
+        }
         __syncthreads();
         KAO_PHASE(if (ph) ph[kPhBarrier] = clock64();)
         if (s_abort) return;                                        // a peer vanished: leave, the host reports it
@@ -828,9 +912,9 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // Column-major kernels: X(sync, pop, threads) for every built schedule (kao_set_schedule); each is
 // instantiated for W = 1, 2 and for 32 partition words (compile-time offsets) / any word count.
 #define KAO_FOR_SCHEDULES(X) \
-    X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896) X(4, 0x12, 896) X(2, 0x22, 896)
+    X(1, 0x300, 512) X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896) X(2, 0x22, 896)
 #define KAO_SCHEDULE_DEFAULT_SYNC 1
-#define KAO_SCHEDULE_DEFAULT_POP 0x200
+#define KAO_SCHEDULE_DEFAULT_POP 0x300
 #define KAO_SCHEDULE_DEFAULT_THREADS 512
 #define KAO_PERSISTENT_KERNEL_T(W, NW, S, POP, T)                                                            \
     search_persistent_kernel<EvalCfgT<W, NW, S, POP, T>, T, false>(Params, SmemPlan, uint64_t, uint32_t, uint32_t, \

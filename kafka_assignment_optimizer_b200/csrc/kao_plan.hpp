@@ -68,15 +68,27 @@ inline SmemPlan make_plan(int W, int Ppad, int warps, int obj_words_per_row, int
 // objective table, a batch of candidates per warp (the per-thread generator scans the transposed planes: no inverted lists).
 // mma: the tensor-core form (kao_device_mma.cuh) keeps four shortfall planes behind the rack-field planes
 // (16 nW bytes, at most 4 KB) and has no per-round tables (5,296 bytes): it fits wherever the other form does.
-inline SmemPlan make_plan_t(int W, int Ppad, int threads, int P, int RF, bool mma = false)
+// cands: a sorted-batch schedule (kao_kernels.cuh, build_cand_list) keeps the class histogram, a CTA's share of a
+// round — cands candidate indices sorted by class — and their class bytes behind everything else (at off_inv) if they
+// fit: cand_list_cap(plan) entries, else none.
+constexpr uint32_t kCandClasses = 256;
+inline SmemPlan make_plan_t(int W, int Ppad, int threads, int P, int RF, bool mma = false, uint32_t cands = 0)
 {
     // make_plan sizes the area at off_sw in words per partition of Ppad: the transposed planes hold t_words(Ppad)
     // words per slot, which is Ppad / 32 or (more than 1024 partitions) up to 31 words more — one extra word per
     // partition covers that for every Ppad the evaluator accepts
     const int nW = t_words(Ppad);
     const int per_row = (kTPlanes * W * 32 * nW + Ppad - 1) / Ppad;
-    return make_plan(W, Ppad, threads / 32, per_row, P, RF, false, 32 * batch_stride_words(W), 0,
-                     (kZPlanes + 4 * W + (mma ? 4 : 0)) * nW * 4, !mma);        // term planes + rack-field planes (+ shortfall planes)
+    SmemPlan s = make_plan(W, Ppad, threads / 32, per_row, P, RF, false, 32 * batch_stride_words(W), 0,
+                           (kZPlanes + 4 * W + (mma ? 4 : 0)) * nW * 4, !mma);  // term planes + rack-field planes (+ shortfall planes)
+    const uint64_t need = ((uint64_t)kCandClasses + ((cands + 31u) & ~31ull)) * 5;      // + one class byte per candidate
+    if (mma && cands > 0 && s.total + need <= 227u * 1024u) s.total += (uint32_t)need;
+    return s;
+}
+// entries of the sorted candidate list of a tensor-core plan (0: none, the kernel walks its candidates unsorted)
+__host__ __device__ inline uint32_t cand_list_cap(const SmemPlan &s)
+{
+    return s.total > s.off_inv + kCandClasses * 5 ? (s.total - s.off_inv) / 5 - kCandClasses : 0;
 }
 // does the column-major evaluator cover this layout (kao_create; tests/emu asks the same question)
 inline bool column_major_fits(int W, int Ppad, int threads, int P, int RF)

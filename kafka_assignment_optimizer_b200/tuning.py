@@ -12,8 +12,9 @@ from __future__ import annotations
 import json
 
 # (sync, pop, threads) — the variants csrc/kao_kernels.cuh builds (KAO_FOR_SCHEDULES); the first is the default.
-# pop 0x100: the sums on the tensor cores (binary MMA, csrc/kao_device_mma.cuh); 0x200: the same with the merged generator
-SCHEDULES = [(1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 1024), (4, 0x22, 896), (4, 0x12, 896), (2, 0x22, 896)]
+# pop 0x100: the sums on the tensor cores (binary MMA, csrc/kao_device_mma.cuh); 0x200: the same with the merged generator;
+# 0x300: the same with each CTA's candidates sorted by class (control word) before a round, so a batch runs mostly one body
+SCHEDULES = [(1, 0x300, 512), (1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 1024), (4, 0x22, 896), (2, 0x22, 896)]
 DEFAULT_SCHEDULE = SCHEDULES[0]
 SCHEDULE_FIELDS = ("sync", "pop", "threads")
 

@@ -6,7 +6,8 @@ It builds libkao with -DKAO_PHASE_CLOCKS into a temporary directory (or loads --
 that the kernel records clock64 stamps per warp and round (csrc/kao_kernels.cuh, KAO_PHASE), runs one warm and one
 recorded search on config 3 (1000 x 64 x 8, RF 3) per schedule and prints medians over (CTA, warp, round):
 generate + park and eval_batch_mma per batch, and per round the work, the wait at the CTA reduce, the grid
-barrier, the winner's re-materialisation and patch, and rebuild_lists.  The stamps cost cycles themselves: compare
+barrier, the winner's re-materialisation and patch, and rebuild_lists; with sorted batches also how long warps 1.. take
+to sort the next round's candidates, which they do while warp 0 waits at the grid barrier.  The stamps cost cycles themselves: compare
 the schedules with each other, and take speed from bench.py.  Prints the card's name, power limit and clocks."""
 import argparse
 import os
@@ -16,8 +17,8 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-SLOTS, WARPS, ROUNDS_CAP = 9, 32, 64           # csrc/kao_kernels.cuh: kPhSlots, kPhaseWarps, kPhaseRounds
-GEN, EVAL, BATCHES, START, BATCHES_END, REDUCE, BARRIER, APPLY, REBUILD = range(SLOTS)
+SLOTS, WARPS, ROUNDS_CAP = 10, 32, 64          # csrc/kao_kernels.cuh: kPhSlots, kPhaseWarps, kPhaseRounds
+GEN, EVAL, BATCHES, START, BATCHES_END, REDUCE, BARRIER, APPLY, REBUILD, LIST = range(SLOTS)
 
 
 def build_probe_lib(out_dir):
@@ -99,6 +100,9 @@ def main():
             ("round: rebuild_lists", med((w0[:, :, REBUILD] - w0[:, :, APPLY])[ok0])),
             ("round: total (start -> rebuild done)", med((w0[:, :, REBUILD] - w0[:, :, START])[ok0])),
         ]
+        lst = rec[:, LIST] != 0                                           # warps 1.. of a sorted-batch schedule
+        if lst.any():
+            rows.insert(6, ("round: next round sorted, warps 1.. (reduce -> done)", med((rec[lst, LIST] - rec[lst, REDUCE]))))
         for name, v in rows:
             print("  %-46s %10.0f" % (name, v))
     print("SM cycles, medians over (CTA, warp, round); card: %s" % card())
