@@ -255,7 +255,8 @@ int kao_set_evaluator(kao_handle *h, int32_t evaluator);
  * tensor cores instead, one binary MMA over a batch of 32 candidates (kao_device_mma.cuh), and 2 (pop 0x200) does so
  * with a generator whose later operations share their steps across link kinds (fewer divergent paths per warp), and
  * 3 (pop 0x300) does that with every CTA's candidates of a round sorted by the class of their control word first, so
- * that the 32 candidates of a batch mostly take one generator body;
+ * that the 32 candidates of a batch mostly take one generator body, and scores two candidates per instruction in its
+ * MMA epilogue (16 x 2 halfword pairs); a fourth digit 1 (pop 0x1300) keeps that epilogue in 32 bits per candidate;
  * threads per CTA: 512 .. 1024.  Only the six combinations built into the library are accepted (KAO_E_ARG otherwise);
  * the default (1, 0x300, 512) is the fastest one measured on an H100 (config 3; (4, 0x22, 1024) is the fastest popcount one).  Results never depend on it.  The environment variable
  * KAO_SCHEDULE="sync,pop(hex),threads" sets it for every session (and kao_solve); KAO_EVALUATOR=row forces

@@ -49,6 +49,40 @@ inline void ldsm_x4(const uint32_t *row, uint32_t (&a)[4]) { emu_ldsm_x4(row, a)
 inline void bmma_and_popc(int (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) { emu_bmma_and_popc(c, a, b0, b1); }
 #endif
 
+// ------------------------------------------------------------------------------------------
+// 16 x 2 SIMD for the packed epilogue (sorted-batch schedules): per-halfword unsigned max / min, SASS VIMNMX.U16x2,
+// one instruction for two candidates.  The host build (test emulation) restates the CUDA semantics: each halfword of
+// the result is the max / min of the operands' halfwords, no carry or borrow between the halves.
+// ------------------------------------------------------------------------------------------
+#if !defined(KAO_HOST_EMU)
+__device__ __forceinline__ uint32_t vmax16x2(uint32_t a, uint32_t b) { return __vmaxu2(a, b); }
+__device__ __forceinline__ uint32_t vmin16x2(uint32_t a, uint32_t b) { return __vminu2(a, b); }
+#else
+inline uint32_t vmax16x2(uint32_t a, uint32_t b)
+{
+    const uint32_t al = a & 0xFFFFu, bl = b & 0xFFFFu, ah = a >> 16, bh = b >> 16;
+    return (al > bl ? al : bl) | (ah > bh ? ah : bh) << 16;
+}
+inline uint32_t vmin16x2(uint32_t a, uint32_t b)
+{
+    const uint32_t al = a & 0xFFFFu, bl = b & 0xFFFFu, ah = a >> 16, bh = b >> 16;
+    return (al < bl ? al : bl) | (ah < bh ? ah : bh) << 16;
+}
+#endif
+// a slot's bounds lo | hi << 16 clamped to P (PP = P | P << 16): lo' and hi' each in both halves
+__device__ __forceinline__ void bounds16x2(uint32_t b, uint32_t PP, uint32_t &lo2, uint32_t &hi2)
+{
+    const uint32_t bc = vmin16x2(b, PP);
+    lo2 = __byte_perm(bc, 0u, 0x1010);
+    hi2 = __byte_perm(bc, 0u, 0x3232);
+}
+// what the clamp leaves to a per-launch constant: max(lo - P, 0) - min(hi, P)
+__device__ __forceinline__ int bounds16x2_rest(uint32_t b, uint32_t PP)
+{
+    const uint32_t bc = vmin16x2(b, PP);
+    return (int)((b - bc) & 0xFFFFu) - (int)(bc >> 16);
+}
+
 // one word (32 partitions) of shortfall plane k: bit k of max(0, RF - replicas of the row), 0 beyond P
 template <int W>
 __device__ __forceinline__ uint32_t s_gather(const Params &d, int k, int w, const uint32_t *bitsT)
@@ -231,29 +265,68 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     int v[8], o[8], rpen[2] = {0, 0};
 #pragma unroll
     for (int e = 0; e < 8; ++e) v[e] = o[e] = 0;
+    // Packed epilogue (Cfg::kPacked: pop 0x300; 0x1300 keeps the 32-bit form below): d0 / d1 of a lane are candidates 2 t and 2 t + 1 of one slot row, so the pair
+    // travels as one register x = x0 | x1 << 16 (PRMT) and its delta bytes are spread into the two halves.  Every
+    // column total is 0 <= c <= P <= 8,160, and with the bounds clamped to lo' = min(lo, P), hi' = min(hi, P)
+    //     max(c - hi, 0) + max(lo - c, 0) = max(c, hi') + max(c, lo') - c  - hi' + (lo - lo')        (c <= P)
+    // so a slot costs two VIMNMX.U16x2 per pair, and - hi' + (lo - lo') summed over the slots is one constant of the
+    // launch, added at the end (one warp reduction per batch).
+    // The pair sums r = lo + hi << 16 of an m-tile are plain 32-bit adds: each half's total stays in 0 .. 65,535 (bounds
+    // at the loops), so no carry crosses the halves.  They widen once per m-tile: v[2 nt] sums r and v[2 nt + 1] sums
+    // r >> 16 (one IADD, one LEA.HI); after the last m-tile v[2 nt] - (v[2 nt + 1] << 16) is the sum of the low halves,
+    // exact mod 2^32, and that sum is far below 2^31.
+    const uint32_t PP = (uint32_t)d.P * 0x10001u;
+    auto widen = [&](const uint32_t (&r)[4]) {
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) { v[2 * nt] = (int)((uint32_t)v[2 * nt] + r[nt]); v[2 * nt + 1] += (int)(r[nt] >> 16); }
+    };
+    auto pair = [&](int nt, int h) { return __byte_perm((uint32_t)acc[nt][2 * h], (uint32_t)acc[nt][2 * h + 1], 0x5410); };
+    // delta nibbles (masked to the low nibble of each byte) of candidates 8 nt + 2 t, + 1: bytes 2 nt, 2 nt + 1 of the row
+    auto spread = [](uint32_t nx, uint32_t ny, int nt) { return __byte_perm(nt < 2 ? nx : ny, 0u, (nt & 1) ? 0x4342 : 0x4140); };
     // ---- replicas: 2 D (rows), C3, and the rack totals (C6)
 #pragma unroll 1
     for (int mt = 0; mt < 2 * W; ++mt) {
         const int s = 16 * mt + lrow;
         tile(T + (size_t)(0 * NSL + s) * nW, swz ? 4 * (s & 7) : 0);
         int rk[8];
+        if constexpr (Cfg::kPacked) {
+            // per half and slot: 2 D + the C3 terms = max(c, hi') + max(c, lo') + D - delta, in 2 D .. 3 P; two slots
+            // <= 6 P = 48,960
+            uint32_t r[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int sl = 16 * mt + 8 * h + g;
-            const uint32_t b = cs->bnd_rep[sl];
-            const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
-            const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+            for (int h = 0; h < 2; ++h) {
+                const int sl = 16 * mt + 8 * h + g;
+                uint32_t lo2, hi2;
+                bounds16x2(cs->bnd_rep[sl], PP, lo2, hi2);
+                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+                const uint32_t nx = nb.x & 0x0F0F0F0Fu, ny = nb.y & 0x0F0F0F0Fu;
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    const int e = 2 * nt + jj;
-                    const int dd = acc[nt][2 * h + jj];
-                    const int c = dd + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3))) & 15u);
-                    v[e] += 2 * dd + max(c - hi, 0) + max(lo - c, 0);
-                    if (jj == 0) rk[4 * h + nt] = c;
-                    else rk[4 * h + nt] |= c << 16;             // c <= P < 8192: a rack's 8 slots stay below 2^16
+                for (int nt = 0; nt < 4; ++nt) {
+                    const uint32_t d2 = pair(nt, h), n2 = spread(nx, ny, nt), c2 = d2 + n2;
+                    r[nt] += vmax16x2(c2, hi2) + vmax16x2(c2, lo2) + d2 - n2;
+                    rk[4 * h + nt] = (int)c2;                       // c <= P < 8192: a rack's 8 slots stay below 2^16
                 }
+            }
+            widen(r);
+        } else {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int sl = 16 * mt + 8 * h + g;
+                const uint32_t b = cs->bnd_rep[sl];
+                const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
+                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                    for (int jj = 0; jj < 2; ++jj) {
+                        const int e = 2 * nt + jj;
+                        const int dd = acc[nt][2 * h + jj];
+                        const int c = dd + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3))) & 15u);
+                        v[e] += 2 * dd + max(c - hi, 0) + max(lo - c, 0);
+                        if (jj == 0) rk[4 * h + nt] = c;
+                        else rk[4 * h + nt] |= c << 16;         // c <= P < 8192: a rack's 8 slots stay below 2^16
+                    }
+            }
         }
         // rack totals: the 8 slots of a rack are the 8 lane groups; lane (g, t) gets rack 2 mt + (g >> 2) of candidates
         // 8 (g & 3) + 2 t + jj
@@ -269,21 +342,47 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     for (int mt = 0; mt < 2 * W; ++mt) {
         const int s = 16 * mt + lrow;
         tile(T + (size_t)(1 * NSL + s) * nW, swz ? 4 * (s & 7) : 0);
+        if constexpr (Cfg::kPacked) {
+            // per half and slot: the C4 terms - l = max(l, hi') + max(l, lo') - 2 l, in 0 .. 2 P; two slots <= 4 P = 32,640
+            uint32_t m[4] = {0u, 0u, 0u, 0u}, ls[4] = {0u, 0u, 0u, 0u}, r[4];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int sl = 16 * mt + 8 * h + g;
-            const uint32_t b = cs->bnd_ldr[sl];
-            const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
-            const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+            for (int h = 0; h < 2; ++h) {
+                const int sl = 16 * mt + 8 * h + g;
+                uint32_t lo2, hi2;
+                bounds16x2(cs->bnd_ldr[sl], PP, lo2, hi2);
+                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+                const uint32_t nx = (nb.x >> 4) & 0x0F0F0F0Fu, ny = (nb.y >> 4) & 0x0F0F0F0Fu;
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    const int e = 2 * nt + jj;
-                    const int l = acc[nt][2 * h + jj] + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3) + 4)) & 15u);
-                    v[e] += max(l - hi, 0) + max(lo - l, 0) - l;
+                for (int nt = 0; nt < 4; ++nt) {
+                    const uint32_t l2 = pair(nt, h) + spread(nx, ny, nt);
+                    m[nt] += vmax16x2(l2, hi2) + vmax16x2(l2, lo2);
+                    ls[nt] += l2;
                 }
+            }
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) r[nt] = m[nt] - 2u * ls[nt];
+            widen(r);
+        } else {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int sl = 16 * mt + 8 * h + g;
+                const uint32_t b = cs->bnd_ldr[sl];
+                const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
+                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                    for (int jj = 0; jj < 2; ++jj) {
+                        const int e = 2 * nt + jj;
+                        const int l = acc[nt][2 * h + jj] + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3) + 4)) & 15u);
+                        v[e] += max(l - hi, 0) + max(lo - l, 0) - l;
+                    }
+            }
         }
+    }
+    if constexpr (Cfg::kPacked) {
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) v[2 * nt] = (int)((uint32_t)v[2 * nt] - ((uint32_t)v[2 * nt + 1] << 16));
     }
     // ---- term planes (objective), rack-field planes (- z) and shortfall planes (+ 2 * 2^k): rows Z[0..8 + 4 W + 4),
     // one tile at W = 1, two at W = 2 (the second one's rows beyond the shortfall planes repeat them and weigh nothing)
@@ -316,6 +415,12 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     const uint4 h = *reinterpret_cast<const uint4 *>(batch + mma_lane_candidate(lane) * kBatchHdr);
     viol_out = viol + (int)h.z + d.P - d.RF * (d.P - (int)(h.y >> 16));
     obj_out = obj + (int)h.w;
+    if constexpr (Cfg::kPacked) {                                  // the clamp's constant, over every slot of both tables
+        int k = 0;
+#pragma unroll
+        for (int sl = lane; sl < NSL; sl += 32) k += bounds16x2_rest(cs->bnd_rep[sl], PP) + bounds16x2_rest(cs->bnd_ldr[sl], PP);
+        viol_out += __reduce_add_sync(0xFFFFFFFFu, k);
+    }
 }
 
 }  // namespace kao

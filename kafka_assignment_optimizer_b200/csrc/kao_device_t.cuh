@@ -48,12 +48,16 @@ namespace kao {
 //              a third hex digit picks where the sums are formed: 0 = the popcount streams above, 1 = on the tensor
 //              cores, a binary MMA over a batch of 32 candidates (kao_device_mma.cuh; the two low digits and kSync
 //              then play no part)
+//              with the third digit 3 the MMA epilogue scores two candidates per instruction in 16 x 2 halfword pairs
+//              (kao_device_mma.cuh, eval_batch_mma); a fourth hex digit 1 keeps it in 32 bits per candidate
 //   kThreads   threads per CTA (0 = threads_for<W>()); fewer threads = more registers per thread
 template <int W_, int kNW_ = 0, int kSync_ = 1, int kPop_ = 0x22, int kThreads_ = 0>
 struct EvalCfgT {
     static constexpr int W = W_, NPH = 5, kRack = 3, kObj = 3, kNW = kNW_;
     static constexpr int kSync = kSync_, kPop = kPop_, kThreads = kThreads_;
-    static constexpr int kSums = kPop_ >> 8;
+    static constexpr int kSums = (kPop_ >> 8) & 15;
+    static constexpr bool kPacked = kSums == 3 && !((kPop_ >> 12) & 1);
+    static_assert(!((kPop_ >> 12) & 1) || kSums == 3, "the 32-bit epilogue digit applies to the sorted-batch body");
     static constexpr bool kTrans = true;
 };
 constexpr int kTPlanes = 2;

@@ -912,7 +912,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // Column-major kernels: X(sync, pop, threads) for every built schedule (kao_set_schedule); each is
 // instantiated for W = 1, 2 and for 32 partition words (compile-time offsets) / any word count.
 #define KAO_FOR_SCHEDULES(X) \
-    X(1, 0x300, 512) X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896) X(2, 0x22, 896)
+    X(1, 0x300, 512) X(1, 0x1300, 512) X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896)
 #define KAO_SCHEDULE_DEFAULT_SYNC 1
 #define KAO_SCHEDULE_DEFAULT_POP 0x300
 #define KAO_SCHEDULE_DEFAULT_THREADS 512

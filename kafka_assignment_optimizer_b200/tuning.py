@@ -13,8 +13,10 @@ import json
 
 # (sync, pop, threads) — the variants csrc/kao_kernels.cuh builds (KAO_FOR_SCHEDULES); the first is the default.
 # pop 0x100: the sums on the tensor cores (binary MMA, csrc/kao_device_mma.cuh); 0x200: the same with the merged generator;
-# 0x300: the same with each CTA's candidates sorted by class (control word) before a round, so a batch runs mostly one body
-SCHEDULES = [(1, 0x300, 512), (1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 1024), (4, 0x22, 896), (2, 0x22, 896)]
+# 0x300: the same with each CTA's candidates sorted by class (control word) before a round, so a batch runs mostly one body,
+# and the MMA epilogue scoring two candidates per instruction in 16 x 2 halfword pairs; 0x1300: the same with the epilogue
+# in 32 bits per candidate
+SCHEDULES = [(1, 0x300, 512), (1, 0x1300, 512), (1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 1024), (4, 0x22, 896)]
 DEFAULT_SCHEDULE = SCHEDULES[0]
 SCHEDULE_FIELDS = ("sync", "pop", "threads")
 
