@@ -133,16 +133,125 @@ for _regime, (_f, _bases) in _REGIMES.items():
         LAYOUT_SHAPES["%s_%s" % (_regime, _b)] = (lambda f=_f, b=_b, seed=60 + _i: f({**SHAPES, **LAYOUT_SHAPES}[b](), seed))
 
 
-def ragged_problem():
-    import numpy as np
-
-    rng = np.random.RandomState(12)
+def ragged_problem(P=60, seed=12):
+    rng = np.random.RandomState(seed)
     B0, removed = 14, 3
     current = []
-    for p in range(60):
+    for p in range(P):
         k = 1 + p % 4
         current.append(list(map(int, rng.choice(B0, size=k, replace=False))))
-    current[5] = [12, 13]                 # every replica on a broker that leaves the cluster
+    for p in range(5, P, 997):
+        current[p] = [12, 13]             # every replica on a broker that leaves the cluster
     current[6] = [11]
     racks = {b: "az%d" % (b % 3) for b in range(B0)}
     return m.build_problem(current, list(range(B0 - removed)), racks, 3)
+
+
+# ---- the HBM-base search path (DESIGN.md 7.1): every topic session and every instance above 8,160 partitions
+# Its evaluator is the general-bounds form at every rack width, so the C7 form (at most one replica per rack 0..1,
+# exactly one 1..1, or a lower bound above 0 with RF > racks) is a layout axis of its own there.  Small shapes for the
+# (row width, rack field, C7 form) combinations the shapes above leave out, each with packed entries and a dense table.
+_C7_LAYOUTS = {
+    "c7_w1_s8_lo": ([6, 6, 6], 4),          # C7 1..2
+    "c7_w1_s16_lo": ([10, 10], 3),          # C7 1..2
+    "c7_w1_word_11": ([20], 1),             # one rack of 20, RF 1: C7 1..1
+    "c7_w1_word_lo": ([20], 2),             # C7 2..2
+    "c7_w2_s8_11": ([6] * 5, 5),
+    "c7_w2_s8_lo": ([6] * 5, 6),
+    "c7_w2_s16_11": ([12, 12, 12], 3),
+    "c7_w2_s16_lo": ([12, 12, 12], 4),
+    "c7_w2_word_11": ([20, 20], 2),
+    "c7_w4_s16_11": ([12] * 5, 5),
+    "c7_w4_s16_lo": ([12] * 5, 6),
+    "c7_w4_word_lo": ([20] * 3, 4),
+    "c7_w8_word_lo": ([40] * 3, 4),
+}
+C7_SHAPES = {}
+for _i, (_n, (_racks, _rf)) in enumerate(sorted(_C7_LAYOUTS.items())):
+    # at most four current replicas: packed entries hold four weighted cells per partition
+    C7_SHAPES[_n] = lambda r=_racks, rf=_rf, s=80 + _i: make_problem(50, r, rf, RFcur=min(rf, 4), seed=s, removed=1)
+    C7_SHAPES[_n + "_dense"] = lambda r=_racks, rf=_rf, s=80 + _i: with_dense_weights(make_problem(50, r, rf, seed=s, removed=1), s)
+
+
+def with_widest_cost_field(pb, seed):
+    """Packed entries with the largest weight the 24-bit objective range allows (floor((2^24 - 1) / (P RF)), present
+    once), seeded weights 1.. that on the current placements: key_obj_bits 24, the narrowest violation field.  Above
+    4,096 partition replicas this is the widest a weight can be (12-bit weights exceed the objective range)."""
+    top = 0xFFFFFF // (pb.P * pb.RF)
+    rng = np.random.RandomState(seed)
+    p, b = np.nonzero(pb.wF | pb.wL)
+    wF, wL = np.zeros(pb.wF.shape, np.int64), np.zeros(pb.wL.shape, np.int64)
+    wF[p, b], wL[p, b] = rng.randint(1, top + 1, size=p.size), rng.randint(1, top + 1, size=p.size)
+    wL[p[0], b[0]] = top
+    return with_weights(pb, wF, wL)
+
+
+def with_saturating_violation(pb, excess=7):
+    """Replica lower bounds raised, broker by broker, until the restatement's initial base violates the rows by the
+    key's violation cap + excess: the first winner is a saturated key."""
+    from oracle import ref
+
+    r = ref.Ref(pb)
+    reps = r.decode(*r.init_base())
+    cap = (1 << (39 - r.obj_bits)) - 1
+    need = cap + excess - m.evaluate(pb, reps)[0]
+    cnt = np.bincount(reps[reps >= 0], minlength=pb.B)
+    lo, hi = pb.rep_lo.copy(), pb.rep_hi.copy()
+    for b in range(pb.B):
+        # broker b's replica term becomes lo - count, its old term (over or under its bounds) plus what is added
+        c = int(cnt[b])
+        old = max(c - int(hi[b]), 0) + max(int(lo[b]) - c, 0)
+        add = min(need, 65535 - c - old)
+        lo[b] = c + old + add
+        hi[b] = max(int(hi[b]), int(lo[b]))
+        need -= add
+    assert need == 0
+    out = dataclasses.replace(pb, rep_lo=lo, rep_hi=hi)
+    assert m.evaluate(out, reps)[0] == cap + excess
+    return out
+
+
+# Above 8,160 partitions only the HBM path runs: the layout edges of SHAPES at those row counts.  Weights above 12 bits
+# have no shape here: P * RF * weight must stay below 2^24, so above 4,096 partition replicas no weight reaches 4,096.
+LARGE_SHAPES = {
+    "big_rf_up": lambda: make_problem(8200, [6, 6, 6], 4, RFcur=2, seed=71),                # RF raised, C7 1..2
+    "big_rf_down": lambda: make_problem(8300, [8, 8, 8, 8], 2, RFcur=4, seed=72),           # four home slots a row
+    "big_ragged": lambda: ragged_problem(8400, seed=73),                                    # 1..4 current replicas
+    "big_rf1": lambda: make_problem(9000, [3, 3, 3], 1, seed=74, removed=1),
+    "big_s64_r1": lambda: make_problem(8300, [40], 3, seed=75),                             # one rack: C7 3..3
+    "big_ppr11_w8": lambda: make_problem(8200, [40, 40, 40], 3, seed=76),                   # eight-word rows, C7 1..1
+    "big_obj24": lambda: with_widest_cost_field(make_problem(8500, [12, 12, 12, 12], 3, seed=77, removed=1), 78),
+    "big_dense_w4": lambda: with_dense_weights(make_problem(8800, [12, 11, 12, 10, 12, 12, 9, 12], 3, seed=79,
+                                                            removed=3), 80),
+    "big_sat": lambda: with_saturating_violation(LARGE_SHAPES["big_obj24"]()),
+}
+
+
+def emptied_base(pb, reps, seed):
+    """A damaged base with rows emptied (their leader byte stays 0xFF: the partitions led from a slot they do not
+    hold), replicas moved to random brokers (duplicates collapse) and rows cut short; the damage scales with P."""
+    rng = np.random.RandomState(seed)
+    out = reps.copy()
+    for p in rng.choice(pb.P, size=max(1, pb.P // 10), replace=False):
+        out[p, rng.randint(pb.RF)] = rng.randint(pb.B)
+    if pb.RF > 1:
+        out[rng.choice(pb.P, size=max(1, pb.P // 30), replace=False), -1] = -1
+    out[rng.choice(pb.P, size=max(1, pb.P // 50), replace=False), :] = -1
+    return out
+
+
+def moved_base(pb, reps, seed):
+    """A damaged base with no row emptied: replicas moved in a quarter of the rows and rows cut short, so that many
+    partitions miss a home broker or are led from elsewhere (long displaced lists)."""
+    rng = np.random.RandomState(seed)
+    out = reps.copy()
+    for p in rng.choice(pb.P, size=max(1, pb.P // 4), replace=False):
+        out[p, rng.randint(pb.RF)] = rng.randint(pb.B)
+        if pb.RF > 1 and rng.randint(2):
+            out[p, ::-1] = out[p].copy()          # another replica leads
+    if pb.RF > 1:
+        cut = rng.choice(pb.P, size=max(1, pb.P // 20), replace=False)
+        out[cut, -1] = -1
+    empty = (out < 0).all(1)
+    out[empty] = reps[empty]                      # a short row that lost its last replica keeps it
+    return out
