@@ -206,6 +206,38 @@ int kao_create(const kao_problem *pb, int32_t device, kao_handle **out);
  * bound (the topic rows only remove assignments), possibly a looser one; optimal = 1 still means proven.  Device
  * memory: 4 bytes per (topic, slot) for the counts (67 MB at 65,280 topics x 256 slots). */
 int kao_create_topics(const kao_problem *pb, const kao_topics *tp, int32_t device, kao_handle **out);
+
+/*
+ * Per-partition replication rows (docs/MODEL.md §11).  kao_problem gives every partition the same C1 (= RF) and C7
+ * (ppr_lo .. ppr_hi per rack); a cluster that mixes RF-3 and RF-2 topics then either raises or lowers a replica count
+ * of every partition of one kind.  A kao_replication REPLACES those two rows, partition by partition:
+ *   C1  sum over brokers of (replica + leader) of p          = rf[p]
+ *   C7  ppr_lo[p] <= sum over the brokers of a rack r of it  <= ppr_hi[p]
+ * pb->RF stays the width of every replica list ([P*RF], -1 padded) and must be >= every rf[p]; pb->ppr_lo / ppr_hi are
+ * still validated but not used.  The initial base (MODEL §4) keeps or completes each row to rf[p].  Every other row,
+ * the objective, the candidate stream and the key layout stay as they are.  Valid input: 1 <= rf[p] <= min(RF, B - 1),
+ * 0 <= ppr_lo[p] <= ppr_hi[p] <= 127, and with topic rows, rep_lo[t] <= the sum of rf over topic t; anything else is
+ * KAO_E_ARG before any CUDA call.  The defaults of the Python binding are ppr = floor / ceil of rf[p] / R.
+ */
+typedef struct kao_replication {
+    const int32_t *rf;                  /* [P] exactly rf[p] replicas */
+    const int32_t *ppr_lo, *ppr_hi;     /* [P] C7 of partition p, per rack */
+} kao_replication;
+
+/* kao_create_topics with the replication rows of `rp` (rp == NULL: exactly kao_create_topics, tp may be NULL).  A
+ * session with `rp` keeps its base in HBM at every P and searches by delta evaluation, as a topic session does, and
+ * refuses what that session refuses (KAO_E_ARG).  kao_get_base returns rows of up to RF entries, -1 padded. */
+int kao_create_replication(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, int32_t device,
+                           kao_handle **out);
+/* kao_solve_topics with the replication rows of `rp` (rp == NULL: exactly kao_solve_topics).  KAO_FLAG_BOUND and the
+ * default bound are the bounds of kao_objective_bound_replication; KAO_FLAG_LP_BOUND with `rp` is KAO_E_ARG. */
+int kao_solve_replication(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp,
+                          const kao_options *opt, kao_result *res);
+/* kao_objective_bound with the replication rows of `rp` (rp == NULL: exactly kao_objective_bound): the cheap bound
+ * takes the best leader plus the best rf[p] - 1 followers; the flow bound has supply rf[p] at partition p and C7 arcs
+ * ppr_lo[p] .. ppr_hi[p].  replicas: a FEASIBLE assignment under those rows, [P*RF], leader first, -1 padded. */
+int kao_objective_bound_replication(const kao_problem *pb, const kao_replication *rp, const int32_t *replicas,
+                                    int64_t *bound);
 int kao_destroy(kao_handle *h);
 /* base <- current assignment restricted to the target brokers and completed to RF (MODEL §4) */
 int kao_reset(kao_handle *h);

@@ -97,12 +97,16 @@ private:
 // the cheap per-partition bound when the flow bound cannot be had (an infeasible start, a runaway).
 inline int64_t objective_flow_bound(const HostModel &m, const kao_problem &pb, const int32_t *replicas, int64_t cheap_bound)
 {
+    // per-partition rows (docs/MODEL.md §11): row p holds rf(p) replicas, the rest of its RF entries are -1
     const int P = m.P, B = m.B, R = m.R, RF = m.RF;
     std::vector<char> y((size_t)P * B, 0);
     std::vector<int> on_broker(B, 0), on_rack(R, 0), led(B, 0), ppr((size_t)P * R, 0);
-    int64_t y_value = 0, l_value = 0;
+    int64_t y_value = 0, l_value = 0, total = 0;
     for (int p = 0; p < P; ++p) {
-        for (int i = 0; i < RF; ++i) {
+        total += m.rf(p);
+        for (int i = m.rf(p); i < RF; ++i)
+            if (replicas[(size_t)p * RF + i] != -1) return cheap_bound;
+        for (int i = 0; i < m.rf(p); ++i) {
             const int b = replicas[(size_t)p * RF + i];
             if (b < 0 || b >= B || y[(size_t)p * B + b]) return cheap_bound;
             y[(size_t)p * B + b] = 1;
@@ -117,10 +121,10 @@ inline int64_t objective_flow_bound(const HostModel &m, const kao_problem &pb, c
     {
         const int S = 0, T = 1, nP = 2, nPR = nP + P, nB = nPR + P * R, nR = nB + B;
         Circulation g(nR + R);
-        g.add(T, S, P * RF, P * RF, 0, P * RF);
+        g.add(T, S, (int)total, (int)total, 0, (int)total);
         for (int p = 0; p < P; ++p) {
-            g.add(S, nP + p, RF, RF, 0, RF);
-            for (int r = 0; r < R; ++r) g.add(nP + p, nPR + p * R + r, m.ppr_lo, m.ppr_hi, 0, ppr[(size_t)p * R + r]);
+            g.add(S, nP + p, m.rf(p), m.rf(p), 0, m.rf(p));
+            for (int r = 0; r < R; ++r) g.add(nP + p, nPR + p * R + r, m.plo(p), m.phi(p), 0, ppr[(size_t)p * R + r]);
             for (int b = 0; b < B; ++b)
                 g.add(nPR + p * R + m.rack_of[b], nB + b, 0, 1, -(int)pb.wF[(size_t)p * B + b], y[(size_t)p * B + b]);
         }

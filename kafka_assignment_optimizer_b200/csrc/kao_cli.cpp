@@ -117,6 +117,8 @@ struct Model {
     // per-topic rows (docs/MODEL.md §10, --topic-balance): topics in name order, floor / ceil of n_t * RF / B and n_t / B
     std::vector<std::string> topic_names;
     std::vector<int32_t> topic_of, trep_lo, trep_hi, tldr_lo, tldr_hi;
+    // per-partition C1 / C7 rows (docs/MODEL.md §11, --keep-rf / --topic-rf): empty when every partition has RF
+    std::vector<int32_t> prf, pprlo, pprhi;
 };
 
 static int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
@@ -181,6 +183,42 @@ Model build_model(std::vector<Row> rows, std::vector<int> brokers, const std::ma
     return m;
 }
 
+// --keep-rf / --topic-rf (docs/MODEL.md §11): every topic keeps the length of its longest replica list (keep_rf, or no
+// --rf given), else takes rf; the topics named in topic_rf take theirs.  When the partitions then differ, RF becomes the
+// largest factor (the width of the replica lists), C3 / C6 and the topic rows follow the sum of the factors and every
+// partition gets its own C1 = rf[p] and C7 = floor / ceil of rf[p] / R; when they agree the model is the plain one.
+Model build_model_rf(const std::vector<Row> &rows, const std::vector<int> &brokers,
+                     const std::map<int, std::string> &racks, bool keep_rf, int rf,
+                     const std::map<std::string, int> &topic_rf)
+{
+    Model m = build_model(rows, brokers, racks, 1);                 // the sorted rows and their topics
+    std::vector<int> longest(m.topic_names.size(), 1);
+    for (int p = 0; p < m.P; ++p) longest[m.topic_of[p]] = std::max(longest[m.topic_of[p]], (int)m.rows[p].replicas.size());
+    for (const auto &kv : topic_rf)
+        if (std::find(m.topic_names.begin(), m.topic_names.end(), kv.first) == m.topic_names.end())
+            throw std::runtime_error("--topic-rf: no topic named " + kv.first + " in the assignment");
+    std::vector<int32_t> prf(m.P);
+    for (int p = 0; p < m.P; ++p) {
+        const std::string &name = m.topic_names[m.topic_of[p]];
+        const auto it = topic_rf.find(name);
+        prf[p] = it != topic_rf.end() ? it->second : (keep_rf || rf <= 0) ? longest[m.topic_of[p]] : rf;
+    }
+    const int top = *std::max_element(prf.begin(), prf.end());
+    m = build_model(rows, brokers, racks, top);
+    if (std::all_of(prf.begin(), prf.end(), [&](int32_t f) { return f == top; })) return m;
+    long tot = 0;
+    std::vector<long> reps(m.topic_names.size(), 0);
+    for (int p = 0; p < m.P; ++p) { tot += prf[p]; reps[m.topic_of[p]] += prf[p]; }
+    std::vector<long> size(m.R, 0);
+    for (int b = 0; b < m.B; ++b) ++size[m.rack_of[b]];
+    m.rep_lo.assign(m.B, (int)(tot / m.B)); m.rep_hi.assign(m.B, ceil_div(tot, m.B));
+    for (int r = 0; r < m.R; ++r) { m.rack_lo[r] = (int)(tot * size[r] / m.B); m.rack_hi[r] = ceil_div(tot * size[r], m.B); }
+    for (size_t t = 0; t < reps.size(); ++t) { m.trep_lo[t] = (int)(reps[t] / m.B); m.trep_hi[t] = ceil_div(reps[t], m.B); }
+    m.prf = prf;
+    for (int32_t f : prf) { m.pprlo.push_back(f / m.R); m.pprhi.push_back(ceil_div(f, m.R)); }
+    return m;
+}
+
 // lp_solve LP-format text, same families and naming as README.md:144-185
 void emit_lp(const Model &m, std::ostream &o, bool topics)
 {
@@ -198,7 +236,7 @@ void emit_lp(const Model &m, std::ostream &o, bool topics)
     o << ";\n\n// Constrain on replication factor for every partition\n";
     for (int p = 0; p < m.P; ++p) {
         for (int b = 0; b < m.B; ++b) o << (b ? " + " : "") << var(b, p, false) << " + " << var(b, p, true);
-        o << " = " << m.RF << ";\n";
+        o << " = " << (m.prf.empty() ? m.RF : m.prf[p]) << ";\n";
     }
     o << "\n// Constraint on having one and only one leader per partition\n";
     for (int p = 0; p < m.P; ++p) {
@@ -232,16 +270,18 @@ void emit_lp(const Model &m, std::ostream &o, bool topics)
         }
     }
     o << "\n// Constrain on min/max replicas per partitions per racks.\n";
-    for (int p = 0; p < m.P; ++p)
+    for (int p = 0; p < m.P; ++p) {
+        const int plo = m.prf.empty() ? m.ppr_lo : m.pprlo[p], phi = m.prf.empty() ? m.ppr_hi : m.pprhi[p];
         for (int r = 0; r < m.R; ++r)
-            for (int pass = 0; pass < (m.ppr_lo > 0 ? 2 : 1); ++pass) {
+            for (int pass = 0; pass < (plo > 0 ? 2 : 1); ++pass) {
                 bool f2 = true;
                 for (int b = 0; b < m.B; ++b) {
                     if (m.rack_of[b] != r) continue;
                     o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true); f2 = false;
                 }
-                o << (pass ? " >= " : " <= ") << (pass ? m.ppr_lo : m.ppr_hi) << ";\n";
+                o << (pass ? " >= " : " <= ") << (pass ? plo : phi) << ";\n";
             }
+    }
     for (int t = 0; topics && t < (int)m.topic_names.size(); ++t)
         for (int kind = 0; kind < 2; ++kind) {
             o << "\n// Constraint on min/max " << (kind ? "leaders" : "replicas") << " of topic " << m.topic_names[t]
@@ -288,7 +328,8 @@ int usage()
 {
     std::fprintf(stderr,
                  "usage: kao-cli --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
-                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--topic-balance] [--emit-lp] [--stats]\n");
+                 "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--topic-balance] [--emit-lp] [--stats]\n"
+                 "               [--keep-rf] [--topic-rf name:N,...]\n");
     return 2;
 }
 
@@ -298,7 +339,7 @@ int main(int argc, char **argv)
 {
     std::map<std::string, std::string> a;
     bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false, lp_certificate = false,
-         topic_balance = false;
+         topic_balance = false, keep_rf = false;
     for (int i = 1; i < argc; ++i) {
         std::string k = argv[i];
         if (k == "--emit-lp") { emit = true; continue; }
@@ -309,6 +350,7 @@ int main(int argc, char **argv)
         if (k == "--certificate") { certificate = true; continue; }  // flow bound: --stats can then say "proven optimal"
         if (k == "--lp-certificate") { lp_certificate = true; continue; }  // Lagrangian LP bound (GPU): proves what the flow bound cannot
         if (k == "--topic-balance") { topic_balance = true; continue; }   // every topic spread over the brokers too
+        if (k == "--keep-rf") { keep_rf = true; continue; }   // every topic keeps its own RF (docs/MODEL.md §11)
         if (k == "--column-major") continue;                  // accepted for old scripts: it is the default now
         if (k.rfind("--", 0) != 0 || i + 1 >= argc) return usage();
         a[k.substr(2)] = argv[++i];
@@ -338,7 +380,15 @@ int main(int argc, char **argv)
         int rf = 0;
         for (auto &r : rows) rf = std::max(rf, (int)r.replicas.size());
         if (a.count("rf")) rf = std::atoi(a["rf"].c_str());
-        Model m = build_model(rows, brokers, racks, rf);
+        std::map<std::string, int> topic_rf;                  // --topic-rf name:N,...
+        for (auto &t : split(a.count("topic-rf") ? a["topic-rf"] : "", ',')) {
+            const size_t c = t.rfind(':');
+            if (c == std::string::npos || c == 0) throw std::runtime_error("--topic-rf entries look like topic:N");
+            topic_rf[t.substr(0, c)] = std::atoi(t.substr(c + 1).c_str());
+        }
+        Model m = keep_rf || !topic_rf.empty()
+                      ? build_model_rf(rows, brokers, racks, keep_rf, a.count("rf") ? rf : 0, topic_rf)
+                      : build_model(rows, brokers, racks, rf);
         if (emit) { emit_lp(m, std::cout, topic_balance); return 0; }
 
         kao_problem pb{};
@@ -365,7 +415,9 @@ int main(int argc, char **argv)
         res.replicas = reps.data();
         kao_topics tp{(int32_t)m.topic_names.size(), m.topic_of.data(), m.trep_lo.data(), m.trep_hi.data(),
                       m.tldr_lo.data(), m.tldr_hi.data()};
-        const int rc = topic_balance ? kao_solve_topics(&pb, &tp, &opt, &res) : kao_solve(&pb, &opt, &res);
+        kao_replication rp{m.prf.data(), m.pprlo.data(), m.pprhi.data()};
+        const int rc = !m.prf.empty() ? kao_solve_replication(&pb, topic_balance ? &tp : nullptr, &rp, &opt, &res)
+                       : topic_balance ? kao_solve_topics(&pb, &tp, &opt, &res) : kao_solve(&pb, &opt, &res);
         if (rc < 0) { std::fprintf(stderr, "kao-cli: %s\n", kao_last_error()); return 1; }
         if (rc == KAO_INFEASIBLE)
             std::fprintf(stderr, "kao-cli: warning: no assignment satisfying every constraint was found (violation %lld)\n",

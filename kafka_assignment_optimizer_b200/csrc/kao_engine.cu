@@ -223,6 +223,9 @@ struct kao_handle {
     // per-topic balance rows (kao_create_topics): always on the large path
     bool topics = false;
     TopicArgs ta{};
+    // per-partition C1 / C7 rows (kao_create_replication): always on the large path, rf | ppr_lo << 8 | ppr_hi << 16
+    bool rf = false;
+    uint32_t *d_rftab = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
 };
@@ -345,7 +348,7 @@ static cudaError_t launch_persistent(kao_handle *h, const PersistArgs &pa, bool 
     if (h->large) {
         ++h->launches;
         return large_search(h->hm.W, h->grid, h->prm, h->la, pa.seed, pa.first_round, pa.rounds, pa.round_size, pa.d_keys,
-                            pa.d_bar, pa.pp, pa.all_keys, pa.st, h->topics ? &h->ta : nullptr);
+                            pa.d_bar, pa.pp, pa.all_keys, pa.st, h->topics ? &h->ta : nullptr, h->d_rftab);
     }
     if (delta) return dispatch(h, LaunchPersistent<true>{}, pa);
     if (h->evaluator == KAO_EVAL_COLUMN_MAJOR) {
@@ -423,12 +426,14 @@ static int reset_impl(kao_handle *h)
     return upload_base(h, bitsT, leader);
 }
 
-static int create_impl(const kao_problem *pb, const kao_topics *tp, int32_t device, kao_handle *h)
+static int create_impl(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, int32_t device,
+                       kao_handle *h)
 {
     std::string why;
     if (!build_host_model(*pb, h->hm, why)) return fail(KAO_E_ARG, why);
+    if (rp && !build_host_replication(*rp, h->hm, why)) return fail(KAO_E_ARG, why);
     HostTopics ht;
-    if (tp && !build_host_topics(*pb, *tp, h->hm.Ppad, ht, why)) return fail(KAO_E_ARG, why);
+    if (tp && !build_host_topics(*pb, *tp, h->hm.Ppad, ht, why, rp ? rp->rf : nullptr)) return fail(KAO_E_ARG, why);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
         return fail(KAO_E_CUDA, "no CUDA device: libkao has no CPU path");
@@ -444,7 +449,8 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, int32_t devi
     const HostModel &m = h->hm;
     const int W = m.W, Ppad = m.Ppad;
     h->topics = tp != nullptr;
-    h->large = m.P > kSmemRowsMax || h->topics;
+    h->rf = rp != nullptr;
+    h->large = m.P > kSmemRowsMax || h->topics || h->rf;
     if (h->large) {
         // the large path scores the objective from packed entries or the dense table (no shared-memory planes)
         h->hm.nplanes = 0;
@@ -506,6 +512,11 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, int32_t devi
         ta.topic_of = topic_of;
         ta.bnd = bnd;
     }
+    if (h->rf) {
+        const std::vector<uint32_t> tab = replication_table(m);
+        CUDA_TRY(dalloc(h, &h->d_rftab, tab.size() * 4));
+        CUDA_TRY(cudaMemcpy(h->d_rftab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
+    }
     CUDA_TRY(dalloc(h, &h->d_nD, 16));
     CUDA_TRY(dalloc(h, &h->d_consts, sizeof(Consts)));
     CUDA_TRY(dalloc(h, &h->d_key, 16));
@@ -546,13 +557,14 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, int32_t devi
     return reset_impl(h);
 }
 
-static int create_handle(const kao_problem *pb, int32_t device, kao_handle **out, const kao_topics *tp = nullptr)
+static int create_handle(const kao_problem *pb, int32_t device, kao_handle **out, const kao_topics *tp = nullptr,
+                         const kao_replication *rp = nullptr)
 {
     if (!pb || !out) return fail(KAO_E_ARG, "null argument");
     *out = nullptr;
     HandleOwner s;
     s.h = new kao_handle();
-    const int rc = create_impl(pb, tp, device, s.h);
+    const int rc = create_impl(pb, tp, rp, device, s.h);
     if (rc == KAO_OK) { *out = s.h; s.h = nullptr; }
     return rc;
 }
@@ -601,7 +613,10 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
     if (violation || objective) {
         if (!h->d_vo) CUDA_TRY(dalloc(h, &h->d_vo, 16));
         int rc = KAO_OK;
-        if (h->topics) {
+        if (h->rf) {
+            CUDA_TRY(large_eval_rf(h->hm.W, h->prm, h->topics ? &h->ta : nullptr, h->d_rftab, h->d_vo, h->d_vo + 1, 0));
+            ++h->launches;
+        } else if (h->topics) {
             CUDA_TRY(large_eval_topics(h->hm.W, h->prm, h->ta, h->d_vo, h->d_vo + 1, 0));
             ++h->launches;
         } else {
@@ -618,8 +633,13 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
 
 // what a session of more than kSmemRowsMax partitions does not offer (kao.h): full per-candidate evaluation, the choice
 // of full evaluator, and sharding one search over several GPUs
-static int refuse_large(const char *what, bool topics = false)
+static int refuse_large(const char *what, bool topics = false, bool rf = false)
 {
+    if (rf)
+        return fail(KAO_E_ARG, std::string(what) + ": not offered with per-partition replication factors "
+                                                   "(kao_create_replication / kao_solve_replication keep the base and "
+                                                   "the per-partition rows in HBM and search with delta evaluation on "
+                                                   "one GPU per search, at every P)");
     if (topics)
         return fail(KAO_E_ARG, std::string(what) + ": not offered with topic rows (kao_create_topics / kao_solve_topics "
                                                    "keep the base and the per-topic counts in HBM and search with delta "
@@ -645,7 +665,8 @@ static int check_search_args(const kao_handle *h, uint32_t rounds, uint32_t roun
 {
     if (h && h->large && !delta)
         return fail(KAO_E_ARG, std::string("full per-candidate evaluation is not offered ") +
-                                   (h->topics ? "with topic rows" : "above 8,160 partitions") +
+                                   (h->rf ? "with per-partition replication factors"
+                                          : h->topics ? "with topic rows" : "above 8,160 partitions") +
                                    ": use delta evaluation (kao_search_delta, kao_candidate_keys_delta)");
     if (rounds > KAO_MAX_ROUNDS) return fail(KAO_E_ARG, "rounds must not exceed KAO_MAX_ROUNDS (2^20) per call");
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "round_size must be 2..2^24");
@@ -783,7 +804,7 @@ static int publish_mailboxes(kao_handle *h, int rank, int world)
 static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 {
     if (!h || !handle_out) return fail(KAO_E_ARG, "null argument");
-    if (h->large) return refuse_large("kao_p2p_export", h->topics);
+    if (h->large) return refuse_large("kao_p2p_export", h->topics, h->rf);
     static_assert(sizeof(cudaIpcMemHandle_t) == KAO_IPC_HANDLE_BYTES, "ipc handle size");
     const int rc = ensure_mailbox(h);
     if (rc != KAO_OK) return rc;
@@ -796,7 +817,7 @@ static int p2p_export_impl(kao_handle *h, uint8_t *handle_out)
 static int p2p_connect_impl(kao_handle *h, int32_t rank, int32_t world, const uint8_t *handles)
 {
     if (!h || !handles) return fail(KAO_E_ARG, "null argument");
-    if (h->large) return refuse_large("kao_p2p_connect", h->topics);
+    if (h->large) return refuse_large("kao_p2p_connect", h->topics, h->rf);
     if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(KAO_E_ARG, "bad rank / world");
     if (!h->d_mail) return fail(KAO_E_STATE, "call kao_p2p_export first");
     CUDA_TRY(cudaSetDevice(h->device));
@@ -816,7 +837,7 @@ static int sharded_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint
                         uint32_t round_size, uint64_t *round_keys, double *device_ms, bool delta)
 {
     if (!h) return fail(KAO_E_ARG, "null handle");
-    if (h->large) return refuse_large("sharded search", h->topics);
+    if (h->large) return refuse_large("sharded search", h->topics, h->rf);
     const int rc = check_search_args(h, rounds, round_size, delta);
     if (rc != KAO_OK) return rc;
     if (h->p2p_world < 2 || !h->peer_mail[h->p2p_world - 1]) return fail(KAO_E_STATE, "kao_p2p_connect first");
@@ -862,7 +883,7 @@ static int profile_rounds_impl(kao_handle *h, uint64_t seed, uint32_t first_roun
                                uint32_t round_size, double *search_ms, double *apply_ms)
 {
     if (!h || !rounds || rounds > 4096) return fail(KAO_E_ARG, "bad argument (1..4096 rounds)");
-    if (h->large) return refuse_large("kao_profile_rounds (full evaluation, one launch per round)", h->topics);
+    if (h->large) return refuse_large("kao_profile_rounds (full evaluation, one launch per round)", h->topics, h->rf);
     if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
     CUDA_TRY(cudaSetDevice(h->device));
     struct Events {
@@ -1138,15 +1159,16 @@ static int solve_gang(const kao_problem *pb, const kao_options *opt, const std::
 // The restarts side by side on the GPUs of the call: restart r runs on GPU r mod N as an ordinary single-GPU search
 // (no exchange between the GPUs at all), one host thread per GPU and none for one GPU.  The winner is exactly what
 // one GPU returns for the same call: this is kao_solve on one GPU, and with KAO_FLAG_SPREAD_RESTARTS on several.
-static int solve_restarts(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, const std::vector<int> &devs,
-                          uint32_t restarts, bool delta, std::chrono::steady_clock::time_point t0, Solved &out)
+static int solve_restarts(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, const kao_options *opt,
+                          const std::vector<int> &devs, uint32_t restarts, bool delta,
+                          std::chrono::steady_clock::time_point t0, Solved &out)
 {
     const int world = (int)devs.size();
     std::vector<Solved> per(world);
     const int rc = on_each_gpu(devs, [&](int i) {
         Solved &g = per[i];
         HandleOwner s;
-        int rc = create_handle(pb, devs[i], &s.h, tp);
+        int rc = create_handle(pb, devs[i], &s.h, tp, rp);
         if (rc != KAO_OK) return rc;
         stamp(t0, "session created (model built, tables uploaded, initial base)");
         kao_handle *h = s.h;
@@ -1178,24 +1200,31 @@ static int solve_restarts(const kao_problem *pb, const kao_topics *tp, const kao
     return KAO_OK;
 }
 
-static int solve_impl(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, kao_result *res)
+static int solve_impl(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, const kao_options *opt,
+                      kao_result *res)
 {
     if (!pb || !opt || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
     int rc = check_search_args(nullptr, opt->rounds, opt->round_size, false);
     if (rc != KAO_OK) return rc;
-    if (tp) {
-        // the topic rows are checked before any CUDA call (each session builds them again)
+    if (tp || rp) {
+        // the topic and replication rows are checked before any CUDA call (each session builds them again)
         HostModel m;
         HostTopics ht;
         std::string why;
-        if (!build_host_model(*pb, m, why) || !build_host_topics(*pb, *tp, m.Ppad, ht, why)) return fail(KAO_E_ARG, why);
+        if (!build_host_model(*pb, m, why) || (rp && !build_host_replication(*rp, m, why)) ||
+            (tp && !build_host_topics(*pb, *tp, m.Ppad, ht, why, rp ? rp->rf : nullptr)))
+            return fail(KAO_E_ARG, why);
     }
-    // more than kSmemRowsMax partitions, or topic rows: the large path, which searches with delta evaluation (kao_solve
-    // returns the assignment, whatever evaluator found it) on one GPU per search; refused before anything is searched
-    const bool large = pb->P > kSmemRowsMax || tp;
+    if (rp && (opt->flags & KAO_FLAG_LP_BOUND))
+        return fail(KAO_E_ARG, "KAO_FLAG_LP_BOUND: the Lagrangian LP bound is built for one RF and one C7 row for every "
+                               "partition (docs/MODEL.md 9), not for per-partition replication factors");
+    // more than kSmemRowsMax partitions, topic rows or replication rows: the large path, which searches with delta
+    // evaluation (kao_solve returns the assignment, whatever evaluator found it) on one GPU per search; refused before
+    // anything is searched
+    const bool large = pb->P > kSmemRowsMax || tp || rp;
     const bool sharded = (opt->n_gpus > 1 || __builtin_popcount(opt->device_mask) > 1) && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS);
-    if (large && (opt->flags & KAO_FLAG_ROW_MAJOR)) return refuse_large("KAO_FLAG_ROW_MAJOR", tp);
-    if (large && sharded) return refuse_large("n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS (every round sharded over the GPUs)", tp);
+    if (large && (opt->flags & KAO_FLAG_ROW_MAJOR)) return refuse_large("KAO_FLAG_ROW_MAJOR", tp, rp);
+    if (large && sharded) return refuse_large("n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS (every round sharded over the GPUs)", tp, rp);
     if ((opt->flags & KAO_FLAG_LP_BOUND) && !lp_bound_fits(*pb)) return fail(KAO_E_ARG, std::string("KAO_FLAG_LP_BOUND: ") + kLpLimit);
     const auto t0 = std::chrono::steady_clock::now();
     std::vector<int> devs;
@@ -1208,7 +1237,7 @@ static int solve_impl(const kao_problem *pb, const kao_topics *tp, const kao_opt
     const bool delta = (opt->flags & KAO_FLAG_DELTA) != 0 || large;
     Solved s;
     rc = world > 1 && !(opt->flags & KAO_FLAG_SPREAD_RESTARTS) ? solve_gang(pb, opt, devs, restarts, delta, s)
-                                                                : solve_restarts(pb, tp, opt, devs, restarts, delta, t0, s);
+                                                                : solve_restarts(pb, tp, rp, opt, devs, restarts, delta, t0, s);
     if (rc != KAO_OK) return rc;
     stamp(t0, "session destroyed");
     std::memcpy(res->replicas, s.win.reps.data(), s.win.reps.size() * 4);
@@ -1268,6 +1297,19 @@ extern "C" int kao_objective_bound(const kao_problem *pb, const int32_t *replica
         return KAO_OK;
     });
 }
+extern "C" int kao_objective_bound_replication(const kao_problem *pb, const kao_replication *rp, const int32_t *replicas,
+                                               int64_t *bound)
+{
+    return guarded([&] {
+        if (!pb || !bound) return fail(KAO_E_ARG, "null argument");
+        HostModel m;
+        std::string why;
+        if (!build_host_model(*pb, m, why) || (rp && !build_host_replication(*rp, m, why))) return fail(KAO_E_ARG, why);
+        *bound = objective_upper_bound(m, *pb);
+        if (replicas) *bound = objective_flow_bound(m, *pb, replicas, *bound);
+        return KAO_OK;
+    });
+}
 extern "C" int kao_lp_bound(const kao_problem *pb, const int32_t *replicas, int32_t device, uint32_t max_iterations,
                             int64_t *bound, uint32_t *iterations_run, int64_t *multipliers)
 {
@@ -1293,6 +1335,11 @@ extern "C" int kao_create_topics(const kao_problem *pb, const kao_topics *tp, in
 {
     return guarded([&] { return create_handle(pb, device, out, tp); });
 }
+extern "C" int kao_create_replication(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp,
+                                      int32_t device, kao_handle **out)
+{
+    return guarded([&] { return create_handle(pb, device, out, tp, rp); });
+}
 extern "C" int kao_destroy(kao_handle *h) { return guarded([&] { return destroy_impl(h); }); }
 extern "C" int kao_reset(kao_handle *h) { return guarded([&] { return reset_impl(h); }); }
 extern "C" int kao_set_base(kao_handle *h, const int32_t *replicas) { return guarded([&] { return set_base_impl(h, replicas); }); }
@@ -1305,7 +1352,7 @@ extern "C" int kao_round_launch(kao_handle *h, uint64_t seed, uint32_t round, ui
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
-        if (h->large) return refuse_large("kao_round_launch", h->topics);
+        if (h->large) return refuse_large("kao_round_launch", h->topics, h->rf);
         if (!check_round_args(round_size) || idx_lo > idx_hi || idx_hi > round_size)
             return fail(KAO_E_ARG, "bad round_size / index range");
         CUDA_TRY(cudaSetDevice(h->device));
@@ -1319,7 +1366,7 @@ extern "C" int kao_round_apply(kao_handle *h, uint64_t seed, uint32_t round, uin
 {
     return guarded([&] {
         if (!h || !d_key) return fail(KAO_E_ARG, "null argument");
-        if (h->large) return refuse_large("kao_round_apply", h->topics);
+        if (h->large) return refuse_large("kao_round_apply", h->topics, h->rf);
         if (!check_round_args(round_size)) return fail(KAO_E_ARG, "bad round_size");
         CUDA_TRY(cudaSetDevice(h->device));
         CUDA_TRY(launch_apply(h, seed, round, round_size, reinterpret_cast<const unsigned long long *>(d_key), 0,
@@ -1331,7 +1378,7 @@ extern "C" int kao_set_evaluator(kao_handle *h, int32_t evaluator)
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
-        if (h->large) return refuse_large("kao_set_evaluator", h->topics);
+        if (h->large) return refuse_large("kao_set_evaluator", h->topics, h->rf);
         if (evaluator != KAO_EVAL_ROW_MAJOR && evaluator != KAO_EVAL_COLUMN_MAJOR) return fail(KAO_E_ARG, "unknown evaluator");
         if (evaluator == KAO_EVAL_COLUMN_MAJOR && !h->trans_ok)
             return fail(KAO_E_ARG, "column-major evaluator: needs rows of up to 64 slots, racks of up to 8 brokers, at most one "
@@ -1344,7 +1391,7 @@ extern "C" int kao_set_schedule(kao_handle *h, int32_t sync, int32_t pop, int32_
 {
     return guarded([&] {
         if (!h) return fail(KAO_E_ARG, "null handle");
-        if (h->large) return refuse_large("kao_set_schedule", h->topics);
+        if (h->large) return refuse_large("kao_set_schedule", h->topics, h->rf);
         if (!schedule_exists(sync, pop, threads)) return fail(KAO_E_ARG, "no such schedule (kao.h, kao_set_schedule)");
         h->sch_sync = sync; h->sch_pop = pop; h->sch_threads = threads;
         return KAO_OK;
@@ -1430,9 +1477,14 @@ extern "C" int kao_eval(const kao_problem *pb, int32_t device, const int32_t *re
 }
 extern "C" int kao_solve(const kao_problem *pb, const kao_options *opt, kao_result *res)
 {
-    return guarded([&] { return solve_impl(pb, nullptr, opt, res); });
+    return guarded([&] { return solve_impl(pb, nullptr, nullptr, opt, res); });
 }
 extern "C" int kao_solve_topics(const kao_problem *pb, const kao_topics *tp, const kao_options *opt, kao_result *res)
 {
-    return guarded([&] { return solve_impl(pb, tp, opt, res); });
+    return guarded([&] { return solve_impl(pb, tp, nullptr, opt, res); });
+}
+extern "C" int kao_solve_replication(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp,
+                                     const kao_options *opt, kao_result *res)
+{
+    return guarded([&] { return solve_impl(pb, tp, rp, opt, res); });
 }

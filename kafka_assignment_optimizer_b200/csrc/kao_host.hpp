@@ -45,6 +45,11 @@ struct HostModel {
     std::vector<Cell> cells;                  // all of them, by partition then broker
     std::vector<int> cell_first;              // [P + 1] cells of partition p: cell_first[p] .. cell_first[p + 1]
     std::vector<uint32_t> homeT;              // [Ppad]
+    // per-partition C1 / C7 rows (kao_replication, docs/MODEL.md §11); empty: RF and ppr_lo .. ppr_hi for every row
+    std::vector<uint8_t> rf_p, ppr_lo_p, ppr_hi_p;
+    int rf(int p) const { return rf_p.empty() ? RF : rf_p[p]; }
+    int plo(int p) const { return ppr_lo_p.empty() ? ppr_lo : ppr_lo_p[p]; }
+    int phi(int p) const { return ppr_hi_p.empty() ? ppr_hi : ppr_hi_p[p]; }
 };
 
 inline bool build_host_model(const kao_problem &pb, HostModel &m, std::string &why)
@@ -284,7 +289,7 @@ struct Plane {
 
 // docs/MODEL.md §4: keep what survives of cur (order kept, leader = first survivor, tail dropped
 // beyond RF), then complete short rows greedily: fewest replicas of p in the rack, then least
-// loaded broker, then lowest dense index.
+// loaded broker, then lowest dense index.  With per-partition rows (§11) row p is kept / completed to rf[p].
 inline void initial_base(const HostModel &m, std::vector<uint32_t> &bitsT, std::vector<uint8_t> &leader)
 {
     bitsT.assign((size_t)m.W * m.Ppad, 0);
@@ -292,7 +297,7 @@ inline void initial_base(const HostModel &m, std::vector<uint32_t> &bitsT, std::
     Plane pl{m, bitsT};
     std::vector<int> load(m.B, 0), count(m.P, 0);
     for (int p = 0; p < m.P; ++p) {
-        for (int i = 0; i < m.RFcur && count[p] < m.RF; ++i) {
+        for (int i = 0; i < m.RFcur && count[p] < m.rf(p); ++i) {
             const int b = m.cur[(size_t)p * m.RFcur + i];
             if (b < 0 || pl.has(p, m.slot_of_broker[b])) continue;
             pl.set(p, m.slot_of_broker[b]);
@@ -302,7 +307,7 @@ inline void initial_base(const HostModel &m, std::vector<uint32_t> &bitsT, std::
     }
     std::vector<int> in_rack(m.R);
     for (int p = 0; p < m.P; ++p) {
-        while (count[p] < m.RF) {
+        while (count[p] < m.rf(p)) {
             std::fill(in_rack.begin(), in_rack.end(), 0);
             for (int b = 0; b < m.B; ++b) if (pl.has(p, m.slot_of_broker[b])) ++in_rack[m.rack_of[b]];
             int best = -1;
@@ -370,7 +375,7 @@ inline int count_moves(const HostModel &m, const int32_t *replicas)
 }
 
 // An upper bound on the objective of every feasible assignment: per partition the best choice of a
-// leader plus RF - 1 followers on distinct brokers, with the balance and rack constraints C3..C7
+// leader plus RF - 1 (rf[p] - 1) followers on distinct brokers, with the balance and rack constraints C3..C7
 // dropped.  A search result that reaches it is proven optimal (kao_result.optimal); otherwise the
 // optimum lp_solve would return (README.md:135-136) lies between the two.
 inline int64_t objective_upper_bound(const HostModel &m, const kao_problem &)
@@ -378,9 +383,9 @@ inline int64_t objective_upper_bound(const HostModel &m, const kao_problem &)
     // per partition: the best leader plus the best RF - 1 followers among the other brokers, constraints C3..C7
     // ignored.  Only the non-zero cells matter: every other broker weighs 0 as a follower and as a leader.
     int64_t total = 0;
-    const int nf = m.RF - 1;
     std::vector<std::pair<uint32_t, int>> top;           // follower weights of the row, largest first
     for (int p = 0; p < m.P; ++p) {
+        const int nf = m.rf(p) - 1;
         const int lo = m.cell_first[p], hi = m.cell_first[p + 1];
         top.clear();
         for (int i = lo; i < hi; ++i)
@@ -410,12 +415,14 @@ struct HostTopics {
     std::vector<int32_t> bnd;                 // [T][4]
 };
 
-inline bool build_host_topics(const kao_problem &pb, const kao_topics &tp, int Ppad, HostTopics &ht, std::string &why)
+// rf: the per-partition replication factors of a valid kao_replication (nullptr: RF for every partition)
+inline bool build_host_topics(const kao_problem &pb, const kao_topics &tp, int Ppad, HostTopics &ht, std::string &why,
+                              const int32_t *rf = nullptr)
 {
     auto bad = [&](const std::string &s) { why = "topic rows: " + s; return false; };
     if (tp.T < 1 || tp.T > pb.P) return bad("T must be 1..P");
     if (!tp.topic_of || !tp.rep_lo || !tp.rep_hi || !tp.ldr_lo || !tp.ldr_hi) return bad("null table pointer");
-    std::vector<int64_t> n(tp.T, 0);
+    std::vector<int64_t> n(tp.T, 0), reps(tp.T, 0);
     ht.T = tp.T;
     ht.topic_of.assign((size_t)Ppad, 0);
     for (int p = 0; p < pb.P; ++p) {
@@ -423,18 +430,50 @@ inline bool build_host_topics(const kao_problem &pb, const kao_topics &tp, int P
         if (t < 0 || t >= tp.T) return bad("topic_of[" + std::to_string(p) + "] = " + std::to_string(t) + " is not in 0..T-1");
         ht.topic_of[p] = (uint16_t)t;
         ++n[t];
+        reps[t] += rf ? rf[p] : pb.RF;
     }
     ht.bnd.assign((size_t)tp.T * 4, 0);
     for (int t = 0; t < tp.T; ++t) {
         const int32_t rl = tp.rep_lo[t], rh = tp.rep_hi[t], ll = tp.ldr_lo[t], lh = tp.ldr_hi[t];
         if (rl < 0 || rl > rh || ll < 0 || ll > lh)
             return bad("topic " + std::to_string(t) + ": bounds must satisfy 0 <= lo <= hi");
-        if (rl > n[t] * pb.RF || ll > n[t])
+        if (rl > reps[t] || ll > n[t])
             return bad("topic " + std::to_string(t) + ": lo exceeds what its " + std::to_string(n[t]) +
-                       " partitions can reach (replicas: partitions * RF, leaders: partitions)");
+                       (rf ? " partitions can reach (replicas: the sum of their replication factors, leaders: partitions)"
+                           : " partitions can reach (replicas: partitions * RF, leaders: partitions)"));
         ht.bnd[4 * t] = rl; ht.bnd[4 * t + 1] = rh; ht.bnd[4 * t + 2] = ll; ht.bnd[4 * t + 3] = lh;
     }
     return true;
+}
+
+// The per-partition C1 / C7 rows of a kao_replication (docs/MODEL.md §11) into m (built by build_host_model):
+// 1 <= rf[p] <= min(RF, B - 1), 0 <= ppr_lo[p] <= ppr_hi[p] <= 127.
+inline bool build_host_replication(const kao_replication &rp, HostModel &m, std::string &why)
+{
+    auto bad = [&](const std::string &s) { why = "per-partition replication factors: " + s; return false; };
+    if (!rp.rf || !rp.ppr_lo || !rp.ppr_hi) return bad("null table pointer");
+    const int top = std::min(m.RF, m.B - 1);
+    m.rf_p.assign((size_t)m.P, 0);
+    m.ppr_lo_p.assign((size_t)m.P, 0);
+    m.ppr_hi_p.assign((size_t)m.P, 0);
+    for (int p = 0; p < m.P; ++p) {
+        const int32_t f = rp.rf[p], lo = rp.ppr_lo[p], hi = rp.ppr_hi[p];
+        if (f < 1 || f > top)
+            return bad("rf[" + std::to_string(p) + "] = " + std::to_string(f) + " is not in 1.." + std::to_string(top) +
+                       " (the row width RF, and fewer than the brokers)");
+        if (lo < 0 || lo > hi || hi > 127)
+            return bad("partition " + std::to_string(p) + ": per-rack bounds must satisfy 0 <= ppr_lo <= ppr_hi <= 127");
+        m.rf_p[p] = (uint8_t)f; m.ppr_lo_p[p] = (uint8_t)lo; m.ppr_hi_p[p] = (uint8_t)hi;
+    }
+    return true;
+}
+
+// the table the HBM-base kernels read a row's C1 / C7 operands from: rf | ppr_lo << 8 | ppr_hi << 16 per partition
+inline std::vector<uint32_t> replication_table(const HostModel &m)
+{
+    std::vector<uint32_t> t((size_t)m.Ppad, 0);
+    for (int p = 0; p < m.P; ++p) t[p] = (uint32_t)m.rf(p) | ((uint32_t)m.plo(p) << 8) | ((uint32_t)m.phi(p) << 16);
+    return t;
 }
 
 inline void fill_consts(const HostModel &m, Consts &cs)

@@ -50,10 +50,15 @@ cudaError_t large_prepare(int W, const Params &d, const LargeArgs &la, cudaStrea
 cudaError_t topics_prepare(int W, const Params &d, const TopicArgs &ta, cudaStream_t st);
 // rounds first_round .. first_round + rounds - 1 of a delta search in one cooperative launch (one CTA per SM);
 // P2P: rank 0 of 1 (idx_lo / idx_hi, early stop, abort flag, rounds run).  all_keys != nullptr: one round, every
-// candidate's key dumped, the base left as it is.  ta != nullptr: with the topic rows
+// candidate's key dumped, the base left as it is.  ta != nullptr: with the topic rows.  rftab != nullptr: every row's
+// C1 / C7 operands from that per-partition table (docs/MODEL.md §11, replication_table in kao_host.hpp)
 cudaError_t large_search(int W, int grid, const Params &d, const LargeArgs &la, uint64_t seed, uint32_t first_round,
                          uint32_t rounds, uint32_t round_size, unsigned long long *keys, unsigned int *grid_bar,
-                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st, const TopicArgs *ta = nullptr);
+                         const P2P &pp, unsigned long long *all_keys, cudaStream_t st, const TopicArgs *ta = nullptr,
+                         const uint32_t *rftab = nullptr);
+// full evaluation of a replication session's base with its per-partition rows (and its topic rows when ta != nullptr)
+cudaError_t large_eval_rf(int W, const Params &d, const TopicArgs *ta, const uint32_t *rftab, long long *viol,
+                          long long *obj, cudaStream_t st);
 // full evaluation of n explicit assignments (bits [n][W][Ppad], leaders [n][Ppad]): one CTA each
 cudaError_t large_eval(int W, const Params &d, const uint32_t *bits, const uint8_t *leader, int n, long long *viol,
                        long long *obj, cudaStream_t st);

@@ -10,7 +10,7 @@ from typing import Optional
 
 import numpy as np
 
-from .problem import (Problem, TopicRows, build_problem, parse_assignment_json, parse_broker_list, parse_rack_map,
+from .problem import (Problem, ReplicationRows, TopicRows, build_problem, parse_assignment_json, parse_broker_list, parse_rack_map,
                       reassignment_json, topic_rows)
 
 _LIB_PATH = os.environ.get("KAO_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libkao.so")
@@ -94,7 +94,12 @@ def objective_bound(pb: Problem, replicas=None) -> int:
     per-partition bound, or — given a feasible assignment [P, RF], leader first — the flow bound Y* + L*."""
     out = C.c_int64()
     r = None if replicas is None else np.ascontiguousarray(replicas, dtype=np.int32)
-    _check(load_library().kao_objective_bound(_CProblem(pb).ref(), None if r is None else C.c_void_p(r.ctypes.data), C.byref(out)))
+    rp = None if r is None else C.c_void_p(r.ctypes.data)
+    if pb.replication is None:
+        _check(load_library().kao_objective_bound(_CProblem(pb).ref(), rp, C.byref(out)))
+    else:       # per-partition rows: kao_objective_bound_replication (rf[p] replicas per row)
+        cr = _CReplication(pb.replication)
+        _check(load_library().kao_objective_bound_replication(_CProblem(pb).ref(), cr.ref(), rp, C.byref(out)))
     return out.value
 
 
@@ -106,6 +111,9 @@ def lp_bound(pb: Problem, replicas, device: int = 0, max_iterations: int = LP_IT
     """The Lagrangian LP bound of kao_lp_bound (docs/MODEL.md 9; GPU): an upper bound on the objective of every
     feasible assignment, aimed at the objective of `replicas` (a feasible assignment [P, RF], leader first).  -> (bound,
     iterations run), or (bound, iterations run, multipliers int64[2B + R] with LP_FRACTION_BITS fractional bits)."""
+    if pb.replication is not None:
+        raise ValueError("lp_bound: the Lagrangian LP bound is built for one RF and one C7 row for every partition "
+                         "(docs/MODEL.md 9), not for per-partition replication factors")
     r = np.ascontiguousarray(replicas, dtype=np.int32)
     if r.shape != (pb.P, pb.RF):
         raise ValueError("replicas must be [P, RF]")
@@ -154,6 +162,21 @@ class _CTopics:
         return None if self.c is None else C.byref(self.c)
 
 
+class _KaoReplication(C.Structure):
+    _fields_ = [("rf", C.c_void_p), ("ppr_lo", C.c_void_p), ("ppr_hi", C.c_void_p)]
+
+
+class _CReplication:
+    """kao_replication over contiguous copies of a ReplicationRows."""
+
+    def __init__(self, rr: ReplicationRows):
+        self.keep = [np.ascontiguousarray(x, dtype=np.int32) for x in (rr.rf, rr.ppr_lo, rr.ppr_hi)]
+        self.c = _KaoReplication(*(x.ctypes.data for x in self.keep))
+
+    def ref(self):
+        return C.byref(self.c)
+
+
 @dataclasses.dataclass
 class SolveResult:
     replicas: np.ndarray      # int32 [P, RF] dense broker indices, leader first
@@ -174,14 +197,20 @@ class SolveResult:
 
 class Session:
     """Device-resident problem (kao_create .. kao_destroy).  topics: per-topic balance rows (a TopicRows, e.g.
-    topic_rows(pb)) through kao_create_topics; such a session searches with delta evaluation only."""
+    topic_rows(pb)) through kao_create_topics; such a session searches with delta evaluation only.  A problem with
+    per-partition rows (pb.replication, build_problem(keep_rf=...)) opens through kao_create_replication, with or
+    without topics, and also searches with delta evaluation only."""
 
     def __init__(self, pb: Problem, device: int = 0, topics: Optional[TopicRows] = None):
         self.pb = pb
         self._cp = _CProblem(pb)
         self._h = C.c_void_p()
         self._lib = load_library()
-        if topics is None:
+        if pb.replication is not None:
+            self._ct, self._cr = _CTopics(topics), _CReplication(pb.replication)
+            _check(self._lib.kao_create_replication(self._cp.ref(), self._ct.ref(), self._cr.ref(), C.c_int32(device),
+                                                    C.byref(self._h)))
+        elif topics is None:
             _check(self._lib.kao_create(self._cp.ref(), C.c_int32(device), C.byref(self._h)))
         else:
             self._ct = _CTopics(topics)
@@ -346,7 +375,8 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
     result is the same as on one GPU with the same arguments.  tight_bound / lp_bound: objective_bound from the flow
     bound (KAO_FLAG_BOUND) / also from the Lagrangian LP bound (KAO_FLAG_LP_BOUND); either can prove optimality.
     topic_balance: every topic spread over the brokers too (kao_solve_topics with `topics`, by default
-    topic_rows(pb)); the bounds then leave the topic rows out and may be looser."""
+    topic_rows(pb)); the bounds then leave the topic rows out and may be looser.  A problem with per-partition rows
+    (pb.replication) is solved through kao_solve_replication."""
     lib = load_library()
     cp = _CProblem(pb)
     if topic_balance and topics is None:
@@ -357,7 +387,11 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
     opt = _KaoOptions(seed & (2 ** 64 - 1), rounds, round_size, device, flags, n_gpus, device_mask)
     res = _KaoResult()
     res.replicas = reps.ctypes.data
-    if topics is None:
+    if pb.replication is not None:
+        ct, cr = _CTopics(topics), _CReplication(pb.replication)
+        rc = _check(lib.kao_solve_replication(cp.ref(), ct.ref(), cr.ref(), C.byref(opt), C.byref(res)),
+                    allow_infeasible=not require_feasible)
+    elif topics is None:
         rc = _check(lib.kao_solve(cp.ref(), C.byref(opt), C.byref(res)), allow_infeasible=not require_feasible)
     else:
         ct = _CTopics(topics)
@@ -370,7 +404,11 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
 
 def evaluate(pb: Problem, replicas, device: int = 0):
     """GPU evaluation of explicit assignments: replicas [n, P, RF] (or [P, RF]) -> (violation[n],
-    objective[n])."""
+    objective[n]).  Not for a problem with per-partition rows (pb.replication): kao_eval scores C1 / C7 against RF;
+    Session(pb).get_base() evaluates such a problem's base."""
+    if pb.replication is not None:
+        raise ValueError("evaluate: kao_eval scores C1 / C7 against one RF; a problem with per-partition replication "
+                         "factors is evaluated through a Session (set_base, get_base)")
     lib = load_library()
     cp = _CProblem(pb)
     r = np.ascontiguousarray(replicas, dtype=np.int32)
@@ -394,12 +432,15 @@ class AssignmentOptimizer:
         self.seed, self.rounds, self.round_size, self.device = seed, rounds, round_size, device
         self.solve_options = solve_options
 
-    def optimize(self, assignment_json, broker_list, rack_map, rf: Optional[int] = None):
+    def optimize(self, assignment_json, broker_list, rack_map, rf: Optional[int] = None, keep_rf: bool = False,
+                 topic_rf: Optional[dict] = None):
+        """keep_rf: every topic keeps the length of its longest replica list; topic_rf {name: RF}: those topics take
+        that RF, the others keep theirs (keep_rf) or take `rf` (build_problem)."""
         rows, topics = parse_assignment_json(assignment_json)
         brokers = parse_broker_list(broker_list) if isinstance(broker_list, str) else list(broker_list)
         racks = parse_rack_map(rack_map) if isinstance(rack_map, str) else dict(rack_map)
-        if rf is None:
+        if rf is None and not (keep_rf or topic_rf):
             rf = max(len(r) for r in rows)
-        pb = build_problem(rows, brokers, racks, rf, topics)
+        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf)
         res = solve(pb, self.seed, self.rounds, self.round_size, self.device, **self.solve_options)
         return reassignment_json(pb, res.replicas), res

@@ -38,11 +38,22 @@ class Problem:
     cur: np.ndarray         # int32  [P, RFcur] dense indices, -1 = absent
     broker_ids: np.ndarray  # int32  [B]      dense index -> Kafka broker id
     topics: Optional[list] = None   # per-row (topic, partition)
+    replication: Optional["ReplicationRows"] = None   # per-partition C1 / C7 rows (docs/MODEL.md §11), None: RF for all
 
     @classmethod
     def from_fields(cls, other) -> "Problem":
         """Copy any object exposing the same attributes (e.g. the test oracle's Problem)."""
-        return cls(**{f.name: getattr(other, f.name) for f in dataclasses.fields(cls)})
+        return cls(**{f.name: getattr(other, f.name) if f.default is dataclasses.MISSING else getattr(other, f.name, f.default)
+                      for f in dataclasses.fields(cls)})
+
+
+@dataclasses.dataclass
+class ReplicationRows:
+    """Per-partition replication rows (kao_replication, docs/MODEL.md §11): partition p holds exactly rf[p] replicas,
+    and between ppr_lo[p] and ppr_hi[p] of them in every rack.  They replace the problem's C1 (= RF) and C7."""
+    rf: np.ndarray          # int32 [P]
+    ppr_lo: np.ndarray      # int32 [P]
+    ppr_hi: np.ndarray      # int32 [P]
 
 
 def default_weights(cur: np.ndarray, P: int, B: int) -> Tuple[np.ndarray, np.ndarray]:
@@ -70,8 +81,41 @@ def default_bounds(P: int, B: int, R: int, RF: int, rack_of: np.ndarray):
             RF // R, -(-RF // R))
 
 
+def partition_rf(current: Sequence[Sequence[int]], topics: Optional[list], rf: Optional[int], keep_rf: bool = False,
+                 topic_rf: Optional[Dict[str, int]] = None) -> np.ndarray:
+    """The replication factor of every row: with keep_rf (or without `rf`) the length of the longest replica list of its
+    topic, else `rf`; then topic_rf[name] for the topics it names (a name the rows do not contain is a ValueError).
+    Rows without topics form the one topic "t1"."""
+    names = [t[0] if topics else "t1" for t in (topics or [None] * len(current))]
+    longest: Dict[str, int] = {}
+    for name, reps in zip(names, current):
+        longest[name] = max(longest.get(name, 1), len(reps))
+    unknown = sorted(set(topic_rf or {}) - set(longest))
+    if unknown:
+        raise ValueError("topic_rf names topics the assignment does not contain: %s" % ", ".join(unknown))
+    out = np.array([longest[n] if keep_rf or rf is None else int(rf) for n in names], np.int32)
+    for name, n in (topic_rf or {}).items():
+        out[[i for i, t in enumerate(names) if t == name]] = int(n)
+    return out
+
+
 def build_problem(current: Sequence[Sequence[int]], broker_ids: Iterable[int],
-                  rack_by_broker: Dict[int, str], rf: int, topics: Optional[list] = None) -> Problem:
+                  rack_by_broker: Dict[int, str], rf: Optional[int], topics: Optional[list] = None,
+                  keep_rf: bool = False, topic_rf: Optional[Dict[str, int]] = None) -> Problem:
+    """keep_rf / topic_rf (partition_rf): every topic keeps its own replication factor, or takes the one named for it.
+    When the partitions then differ, RF becomes the largest of them (the width of every replica list), C3 / C6 follow
+    from the sum of the per-partition factors and the problem carries per-partition rows (ReplicationRows, C7 = floor /
+    ceil of rf[p] / R); when they all agree the problem is the plain one with that RF."""
+    if keep_rf or topic_rf:
+        rfs = partition_rf(current, topics, rf, keep_rf, topic_rf)
+        pb = build_problem(current, broker_ids, rack_by_broker, int(rfs.max()), topics)
+        if (rfs == rfs[0]).all():
+            return pb
+        tot, size = int(rfs.sum()), np.bincount(pb.rack_of, minlength=pb.R).astype(np.int64)
+        pb.rep_lo, pb.rep_hi = np.full(pb.B, tot // pb.B, np.int32), np.full(pb.B, -(-tot // pb.B), np.int32)
+        pb.rack_lo, pb.rack_hi = ((tot * size) // pb.B).astype(np.int32), (-((-tot * size) // pb.B)).astype(np.int32)
+        pb.replication = ReplicationRows(rfs, (rfs // pb.R).astype(np.int32), (-(-rfs // pb.R)).astype(np.int32))
+        return pb
     ids = sorted({int(b) for b in broker_ids})          # a repeated id is one broker (as kao-cli's build_model)
     dense = {b: i for i, b in enumerate(ids)}
     racks = sorted({str(rack_by_broker[b]) for b in ids})
@@ -133,7 +177,10 @@ def topic_rows(pb: Problem) -> TopicRows:
             names.append(name)
         topic_of[p] = index[name]
     n = np.bincount(topic_of, minlength=len(names)).astype(np.int64)
-    return TopicRows(topic_of, (n * pb.RF // pb.B).astype(np.int32), (-(-n * pb.RF // pb.B)).astype(np.int32),
+    # replicas of each topic: n_t * RF, or the sum of its partitions' factors with per-partition rows
+    reps = n * pb.RF if pb.replication is None else \
+        np.bincount(topic_of, weights=pb.replication.rf, minlength=len(names)).astype(np.int64)
+    return TopicRows(topic_of, (reps // pb.B).astype(np.int32), (-(-reps // pb.B)).astype(np.int32),
                      (n // pb.B).astype(np.int32), (-(-n // pb.B)).astype(np.int32), names)
 
 

@@ -8,7 +8,7 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
                    "racks": "0:a,1:b,...",                               README.md:27-29
                    "rf": 2, "rounds": 256, "round_size": 32768, "restarts": 1, "patience": 0, "delta": false,
                    "gpus": 1, "spread_restarts": false, "certificate": false,
-                   "lp_certificate": false, "topic_balance": false}
+                   "lp_certificate": false, "topic_balance": false, "keep_rf": false, "topic_rf": {}}
     200           {"reassignment": {"version":1,"partitions":[...]},    README.md:67-78
                    "objective": ..., "violation": ..., "moves": ..., "feasible": ...,
                    "objective_bound": ..., "proven_optimal": ...}
@@ -17,7 +17,9 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
 `certificate` asks for the flow bound, so that `proven_optimal` can say the answer is what lp_solve would return
 (README.md:135-136); `lp_certificate` also asks for the Lagrangian LP bound (GPU, docs/MODEL.md §9), which proves
 optima the flow bound cannot, e.g. after brokers are removed.  `topic_balance` also spreads every topic over the
-brokers (the per-topic rows of docs/MODEL.md §10, default bounds of `topic_rows`).
+brokers (the per-topic rows of docs/MODEL.md §10, default bounds of `topic_rows`).  `keep_rf` keeps every topic's own
+replication factor (the length of its longest replica list) and `topic_rf` ({"topic": N}) sets it for the named
+topics, the others keeping theirs or taking `rf` when it is given (per-partition rows, docs/MODEL.md §11).
 
 `python -m kafka_assignment_optimizer_b200.service --port 8080` (needs a GPU: there is no CPU path).
 """
@@ -50,8 +52,15 @@ def handle_submit(body: dict, solver: Optional[Callable] = None) -> dict:
     brokers = parse_broker_list(brokers) if isinstance(brokers, str) else [int(b) for b in brokers]
     racks = body["racks"]
     racks = parse_rack_map(racks) if isinstance(racks, str) else {int(k): str(v) for k, v in racks.items()}
-    rf = int(body.get("rf") or max(len(r) for r in rows))
-    pb = build_problem(rows, brokers, racks, rf, topics)
+    keep_rf, topic_rf = bool(body.get("keep_rf", False)), body.get("topic_rf") or None
+    if keep_rf or topic_rf:
+        # per-partition replication factors (docs/MODEL.md §11): the problem carries them to the solver
+        rf = int(body["rf"]) if body.get("rf") else None
+        topic_rf = {str(k): int(v) for k, v in topic_rf.items()} if topic_rf else None
+        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf)
+    else:
+        rf = int(body.get("rf") or max(len(r) for r in rows))
+        pb = build_problem(rows, brokers, racks, rf, topics)
     if solver is None:
         from .optimizer import solve as solver
     # a request cannot ask for an unbounded search: the limits of include/kao.h, checked here as well
