@@ -1217,10 +1217,23 @@ __device__ void eval_candidate(const Params &d, const uint32_t *bitsT, const uin
 // computed from the base's totals and the candidate's <= 3 patched rows.  One THREAD per candidate.
 // Reported separately from the full-evaluation throughput.
 // ------------------------------------------------------------------------------------------
-// C1 + C7 + leader validity and the objective of ONE row
-template <class Cfg, bool kShared>
+// Per-partition C1 / C7 rows (docs/MODEL.md §11): a replication session reads each row's replica count and per-rack
+// bounds from rftab, one packed word rf | ppr_lo << 8 | ppr_hi << 16 per partition (replication_table in
+// kao_host.hpp; L2-resident, no kernel writes it), instead of Params.
+struct RowRf { int rf, lo, hi; };
+
+__device__ __forceinline__ RowRf row_rf(const uint32_t *rftab, int p)
+{
+    const uint32_t w = __ldg(rftab + p);
+    return {(int)(w & 0xFFu), (int)((w >> 8) & 0xFFu), (int)((w >> 16) & 0xFFu)};
+}
+
+// C1 + C7 + leader validity and the objective of ONE row; kRF: C1 / C7 against r instead of Params.  The Params form
+// stays a branch of its own: routing Params' values through a RowRf changes how nvcc schedules the plain kernels.
+template <class Cfg, bool kShared, bool kRF = false>
 __device__ __forceinline__ void row_eval(const Params &d, const MemRef<kShared> &objT, int p,
-                                         const uint32_t (&x)[Cfg::W], uint32_t ld, int &rv, int &ro)
+                                         const uint32_t (&x)[Cfg::W], uint32_t ld, int &rv, int &ro,
+                                         const RowRf &r = {})
 {
     constexpr int W = Cfg::W;
     uint32_t oh[W], any = 0;
@@ -1231,7 +1244,8 @@ __device__ __forceinline__ void row_eval(const Params &d, const MemRef<kShared> 
         oh[t] = x[t] & lm;
         any |= oh[t];
     }
-    rv = row_rack_terms<W, Cfg::kRack>(x, d.log2S, d.R, d.ppr_lo, d.ppr_hi, d.RF) + (any ? 0 : 1);
+    if constexpr (kRF) rv = row_rack_terms<W, Cfg::kRack>(x, d.log2S, d.R, r.lo, r.hi, r.rf) + (any ? 0 : 1);
+    else rv = row_rack_terms<W, Cfg::kRack>(x, d.log2S, d.R, d.ppr_lo, d.ppr_hi, d.RF) + (any ? 0 : 1);
     ro = 0;
     if constexpr (Cfg::kObj > 0) {
 #pragma unroll
@@ -1306,11 +1320,13 @@ template <int W> __device__ __forceinline__ int lone_slot(const uint32_t (&m)[W]
 // cnt / lcnt: replica and (valid) leader count per slot of the BASE, rc: replica count per rack,
 // base_viol / base_obj: the base's own evaluation.  Every patched partition differs from the base
 // by at most one replica move and/or a leader change (MODEL 5: an op never revisits a partition).
-template <class Cfg, bool kObjShared = true>
+// kRF: every patched row's C1 / C7 operands from rftab, one read per row for its old and its new form.
+template <class Cfg, bool kObjShared = true, bool kRF = false>
 __device__ __forceinline__ void delta_eval(const Params &d, const uint32_t *s_bits, const uint8_t *s_leader,
                                            const MemRef<kObjShared> &objT, const Consts *cs, const PatchSet &ps,
                                            const uint32_t (&rows)[kMaxOps][Cfg::W], const int *cnt, const int *lcnt,
-                                           const int *rc, int base_viol, int base_obj, int &viol, int &obj)
+                                           const int *rc, int base_viol, int base_obj, int &viol, int &obj,
+                                           const uint32_t *rftab = nullptr)
 {
     constexpr int W = Cfg::W;
     viol = base_viol;
@@ -1332,8 +1348,14 @@ __device__ __forceinline__ void delta_eval(const Params &d, const uint32_t *s_bi
             }
             const uint32_t ldo = s_leader[p], ldn = ps.ld[i];
             int rvo, roo, rvn, ron;
-            row_eval<Cfg, kObjShared>(d, objT, p, xo, ldo, rvo, roo);
-            row_eval<Cfg, kObjShared>(d, objT, p, xn, ldn, rvn, ron);
+            if constexpr (kRF) {
+                const RowRf r = row_rf(rftab, p);
+                row_eval<Cfg, kObjShared, true>(d, objT, p, xo, ldo, rvo, roo, r);
+                row_eval<Cfg, kObjShared, true>(d, objT, p, xn, ldn, rvn, ron, r);
+            } else {
+                row_eval<Cfg, kObjShared>(d, objT, p, xo, ldo, rvo, roo);
+                row_eval<Cfg, kObjShared>(d, objT, p, xn, ldn, rvn, ron);
+            }
             viol += rvn - rvo;
             obj += ron - roo;
             es[2 * i] = lone_slot<W>(rem); ev[2 * i] = -1;

@@ -613,11 +613,8 @@ static int get_base_impl(kao_handle *h, int32_t *replicas, int64_t *violation, i
     if (violation || objective) {
         if (!h->d_vo) CUDA_TRY(dalloc(h, &h->d_vo, 16));
         int rc = KAO_OK;
-        if (h->rf) {
-            CUDA_TRY(large_eval_rf(h->hm.W, h->prm, h->topics ? &h->ta : nullptr, h->d_rftab, h->d_vo, h->d_vo + 1, 0));
-            ++h->launches;
-        } else if (h->topics) {
-            CUDA_TRY(large_eval_topics(h->hm.W, h->prm, h->ta, h->d_vo, h->d_vo + 1, 0));
+        if (h->rf || h->topics) {
+            CUDA_TRY(large_eval_base(h->hm.W, h->prm, h->topics ? &h->ta : nullptr, h->d_rftab, h->d_vo, h->d_vo + 1, 0));
             ++h->launches;
         } else {
             rc = eval_on_device(h, h->d_bits, h->d_leader, 1, h->d_vo, h->d_vo + 1);

@@ -30,115 +30,10 @@ template <class T> __device__ __forceinline__ T warp_sum(T v)
     return v;
 }
 
-// ---- per-partition C1 / C7 rows (docs/MODEL.md §11, DESIGN.md §7.3).  A replication session reads each row's replica
-// count and per-rack bounds from rftab, one packed word rf | ppr_lo << 8 | ppr_hi << 16 per partition (L2-resident, no
-// kernel writes it), instead of Params.  row_eval_rf / delta_eval_rf are row_eval / delta_eval (kao_device.cuh) of the
-// large path's configuration (general rack bounds, objective from packed entries or the dense table) with those operands
-// per row; the plain kernels keep calling row_eval / delta_eval themselves.
-struct RowRf { int rf, lo, hi; };
-
-__device__ __forceinline__ RowRf row_rf(const uint32_t *rftab, int p)
-{
-    const uint32_t w = __ldg(rftab + p);
-    return {(int)(w & 0xFFu), (int)((w >> 8) & 0xFFu), (int)((w >> 16) & 0xFFu)};
-}
-
-// C1 + C7 + leader validity and the objective of ONE row, C1 / C7 against r
-template <int W>
-__device__ __forceinline__ void row_eval_rf(const Params &d, const MemRef<false> &objT, int p, const uint32_t (&x)[W],
-                                            uint32_t ld, const RowRf &r, int &rv, int &ro)
-{
-    uint32_t any = 0;
-    const uint32_t ldbit = __funnelshift_l(0u, 1u, ld);
-#pragma unroll
-    for (int t = 0; t < W; ++t) any |= x[t] & (((int)(ld >> 5) == t) ? ldbit : 0u);
-    rv = row_rack_terms<W, LargeCfg<W>::kRack>(x, d.log2S, d.R, r.lo, r.hi, r.rf) + (any ? 0 : 1);
-    ro = 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-        if (k < d.nentries) {
-            const uint32_t e = objT.ld32((uint32_t)(k * d.Ppad + p) * 4u);
-            const uint32_t slot = e & 0xFFu;
-            const uint32_t xw = row_word<W>(x, (int)(slot >> 5));
-            const bool bit = __funnelshift_r(xw, 0u, slot) & 1u;
-            const uint32_t w = (slot == ld) ? (e >> 20) : ((e >> 8) & 0xFFFu);
-            ro += bit ? (int)w : 0;
-        }
-    if (d.dense) {
-        const uint32_t *wrow = d.dense_w + (size_t)p * d.NS;
-#pragma unroll
-        for (int t = 0; t < W; ++t) {
-            for (uint32_t m = x[t]; m; m &= m - 1) {
-                const int s = t * 32 + __ffs(m) - 1;
-                if (s < d.NS) {
-                    const uint32_t w = __ldg(wrow + s);
-                    ro += (s == (int)ld) ? (int)(w >> 16) : (int)(w & 0xFFFFu);
-                }
-            }
-        }
-    }
-}
-
-// delta_eval with every patched row's C1 / C7 operands from rftab (one read per row, for its old and its new form)
-template <int W>
-__device__ __forceinline__ void delta_eval_rf(const Params &d, const uint32_t *rftab, const MemRef<false> &objT,
-                                              const Consts *cs, const PatchSet &ps, const uint32_t (&rows)[kMaxOps][W],
-                                              const int *cnt, const int *lcnt, const int *rc, int base_viol,
-                                              int base_obj, int &viol, int &obj)
-{
-    viol = base_viol;
-    obj = base_obj;
-    int es[2 * kMaxOps], ev[2 * kMaxOps], ls[2 * kMaxOps], lv[2 * kMaxOps];
-#pragma unroll
-    for (int j = 0; j < 2 * kMaxOps; ++j) { es[j] = -1; ev[j] = 0; ls[j] = -1; lv[j] = 0; }
-#pragma unroll
-    for (int i = 0; i < kMaxOps; ++i) {
-        if (i < ps.n) {
-            const int p = ps.p[i];
-            uint32_t xo[W], xn[W], rem[W], add[W];
-#pragma unroll
-            for (int t = 0; t < W; ++t) {
-                xo[t] = d.bitsT[(size_t)t * d.Ppad + p];
-                xn[t] = rows[i][t];
-                rem[t] = xo[t] & ~xn[t];
-                add[t] = xn[t] & ~xo[t];
-            }
-            const uint32_t ldo = d.leader[p], ldn = ps.ld[i];
-            const RowRf r = row_rf(rftab, p);
-            int rvo, roo, rvn, ron;
-            row_eval_rf<W>(d, objT, p, xo, ldo, r, rvo, roo);
-            row_eval_rf<W>(d, objT, p, xn, ldn, r, rvn, ron);
-            viol += rvn - rvo;
-            obj += ron - roo;
-            es[2 * i] = lone_slot<W>(rem); ev[2 * i] = -1;
-            es[2 * i + 1] = lone_slot<W>(add); ev[2 * i + 1] = 1;
-            const bool oko = ((int)ldo < W * 32) && row_has<W>(xo, (int)ldo);
-            const bool okn = ((int)ldn < W * 32) && row_has<W>(xn, (int)ldn);
-            ls[2 * i] = oko ? (int)ldo : -1; lv[2 * i] = -1;
-            ls[2 * i + 1] = okn ? (int)ldn : -1; lv[2 * i + 1] = 1;
-        }
-    }
-    viol += apply_events<2 * kMaxOps>(es, ev, [&](int s, int net) {
-        const uint32_t b = cs->bnd_rep[s];
-        return band_violation(cnt[s] + net, b) - band_violation(cnt[s], b);
-    });
-    viol += apply_events<2 * kMaxOps>(ls, lv, [&](int s, int net) {
-        const uint32_t b = cs->bnd_ldr[s];
-        return band_violation(lcnt[s] + net, b) - band_violation(lcnt[s], b);
-    });
-    int rs[2 * kMaxOps];
-#pragma unroll
-    for (int j = 0; j < 2 * kMaxOps; ++j) rs[j] = es[j] < 0 ? -1 : ((es[j] >> d.log2S) < d.R ? (es[j] >> d.log2S) : -1);
-    viol += apply_events<2 * kMaxOps>(rs, ev, [&](int r, int net) {
-        const int lo = cs->rack_lo[r], hi = cs->rack_hi[r], c0 = rc[r], c1 = rc[r] + net;
-        return (max(c1 - hi, 0) + max(lo - c1, 0)) - (max(c0 - hi, 0) + max(lo - c0, 0));
-    });
-}
-
 // Full evaluation of one assignment by the whole CTA: the per-row terms (C1, C2/C5, C7, objective) of row_eval, the
 // replica and valid-leader count per slot and the replica count per rack in shared memory, then the C3 / C4 / C6
 // bands.  Leaves cnt / lcnt / rc filled (the totals delta evaluation starts from); acc = (violation, objective).
-// rftab != nullptr (kRF): each row's C1 / C7 operands from that table.
+// kRF: each row's C1 / C7 operands from rftab (docs/MODEL.md §11).
 template <int W, bool kRF = false>
 __device__ void block_eval(const Params &d, const Consts *cs, const uint32_t *bits, const uint8_t *leader,
                            int *cnt, int *lcnt, int *rc, long long *acc, const uint32_t *rftab = nullptr)
@@ -155,7 +50,7 @@ __device__ void block_eval(const Params &d, const Consts *cs, const uint32_t *bi
         for (int t = 0; t < W; ++t) x[t] = bits[(size_t)t * d.Ppad + p];
         const uint32_t ld = leader[p];
         int rv, ro;
-        if constexpr (kRF) row_eval_rf<W>(d, m_obj, p, x, ld, row_rf(rftab, p), rv, ro);
+        if constexpr (kRF) row_eval<LargeCfg<W>, false, true>(d, m_obj, p, x, ld, rv, ro, row_rf(rftab, p));
         else row_eval<LargeCfg<W>, false>(d, m_obj, p, x, ld, rv, ro);
         v += rv;
         o += ro;
@@ -422,15 +317,14 @@ __device__ __forceinline__ void apply_winner_topics(const TopicArgs &ta, const C
     }
 }
 
-// the search kernel; kTopics: the topic rows of ta are part of the violation (ta is unused otherwise and comes last,
-// so that the parameters of the plain instantiations are laid out as without it).
-// TWIN: search_large_rf_kernel below repeats this body with per-partition C1 / C7 rows (block_eval<W, true>,
-// delta_eval_rf); any change to the rounds, barriers, early stop, winner or total patching here must be made there too
-// (tests/test_gpu_replication.py compares both with the restatement over multi-round trajectories).
-template <int W, bool kTopics>
+// the search kernel; kTopics: the topic rows of ta are part of the violation; kRF: every row's C1 / C7 operands from
+// rftab ([Ppad] packed words, replication_table in kao_host.hpp; docs/MODEL.md §11).  ta and rftab are unused otherwise
+// and come last, so that the parameters of the plain instantiations are laid out as without them.
+template <int W, bool kTopics, bool kRF>
 __global__ void __launch_bounds__(kLT, 1)
 search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
-                    unsigned long long *keys, unsigned int *grid_bar, P2P pp, unsigned long long *all_keys, TopicArgs ta)
+                    unsigned long long *keys, unsigned int *grid_bar, P2P pp, unsigned long long *all_keys, TopicArgs ta,
+                    const uint32_t *rftab)
 {
     constexpr int kWarps = kLT / 32, NSL = 32 * W;
     __shared__ Consts s_cs;
@@ -457,7 +351,7 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
         // the base's own evaluation and totals: a full pass in the first round; afterwards the totals are patched and
         // the evaluation IS the previous winner's key (unless that key was saturated)
         if (t == 0 || s_base[2] == 0) {
-            block_eval<W>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc);
+            block_eval<W, kRF>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc, rftab);
             if constexpr (kTopics) {
                 if (tid == 0) s_acc[0] += __ldcg(ta.tviol);
             }
@@ -474,159 +368,8 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
                 uint32_t rows[kMaxOps][W];
                 tg.run(seed, round, idx, round_size, ps, rows);
                 int viol, obj;
-                delta_eval<LargeCfg<W>, false>(d, d.bitsT, d.leader, m_obj, &s_cs, ps, rows, s_cnt, s_lcnt, s_rc,
-                                               base_viol, base_obj, viol, obj);
-                if constexpr (kTopics) {
-                    int rc[2 * kMaxOps], lc[2 * kMaxOps];
-                    topic_events<W>(d, ta, &s_cs, ps, rows, rc, lc);
-                    viol += topic_delta<W>(ta, rc, lc);
-                }
-                const unsigned long long key = pack_key(viol, obj, idx, d.key_obj_bits);
-                if (all_keys) all_keys[idx - pp.idx_lo] = key;
-                best = key < best ? key : best;
-            }
-        }
-        if (all_keys) return;                                       // key dump only: the base stays as it is
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, best, o);
-            best = w < best ? w : best;
-        }
-        if (lane == 0) s_red[warp] = best;
-        __syncthreads();
-        if (warp == 0) {
-            unsigned long long v = lane < kWarps ? s_red[lane] : kKeyNone;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, v, o);
-                v = w < v ? w : v;
-            }
-            if (lane == 0) {
-                if (v != kKeyNone) atomicMin(keys + t, v);
-                // grid barrier 1: every CTA's contribution to keys[t] is visible before anyone reads it
-                __threadfence();
-                atomicAdd(grid_bar, 1u);
-                if (!spin_until(grid_bar, (barriers + 1) * gridDim.x, pp.abort, pp.timeout_ns)) s_abort = 1;
-                __threadfence();
-            }
-        }
-        ++barriers;
-        __syncthreads();
-        if (s_abort) return;
-        const unsigned long long k = __ldcg(keys + t);
-        if (tid == 0) {
-            // early stop (the same decision in every CTA: it only depends on the keys)
-            const unsigned long long vc = k >> kIdxBits;
-            if (vc < s_red[kWarps + 1]) { s_red[kWarps + 1] = vc; s_red[kWarps + 2] = 0; } else ++s_red[kWarps + 2];
-            if (pp.patience && s_red[kWarps + 2] >= pp.patience) s_red[kWarps] = 1;
-            if (blockIdx.x == 0 && pp.rounds_run) *pp.rounds_run = t + 1;
-            if (blockIdx.x == 0 && pp.carry) { pp.carry[0] = s_red[kWarps + 1]; pp.carry[1] = s_red[kWarps + 2]; }
-            const uint32_t kv = key_violation(k, d.key_obj_bits);
-            s_base[2] = (k != kKeyNone && (uint64_t)kv < key_viol_cap(d.key_obj_bits)) ? 1 : 0;
-            s_base[0] = (int)kv;
-            s_base[1] = (int)key_objective(k, d.key_obj_bits);
-        }
-        if (k == kKeyNone) {
-            __syncthreads();
-            if (s_red[kWarps]) break;
-            continue;
-        }
-        if (blockIdx.x == 0) apply_winner_large<W>(d, la, &s_cs, s_st, seed, round, round_size, k, s_rec, s_lc);
-        if constexpr (kTopics) {
-            if (blockIdx.x == 0 && tid == 0) apply_winner_topics<W>(ta, &s_cs, s_rec);
-        }
-        // grid barrier 2: the patched HBM state and the winner record are visible before anyone reads them
-        __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            atomicAdd(grid_bar, 1u);
-            if (!spin_until(grid_bar, (barriers + 1) * gridDim.x, pp.abort, pp.timeout_ns)) s_abort = 1;
-            __threadfence();
-        }
-        ++barriers;
-        __syncthreads();
-        if (s_abort) return;
-        if (tid == 0) {
-            // every CTA patches its totals from the record: the old rows out, the new rows in
-            const int n = __ldcg(&la.rec->n);
-            for (int i = 0; i < n; ++i) {
-                for (int t2 = 0; t2 < W; ++t2) {
-                    for (uint32_t m = __ldcg(&la.rec->old_row[i][t2]); m; m &= m - 1) {
-                        const int s = 32 * t2 + __ffs(m) - 1;
-                        --s_cnt[s]; --s_rc[s >> d.log2S];
-                    }
-                    for (uint32_t m = __ldcg(&la.rec->new_row[i][t2]); m; m &= m - 1) {
-                        const int s = 32 * t2 + __ffs(m) - 1;
-                        ++s_cnt[s]; ++s_rc[s >> d.log2S];
-                    }
-                }
-                const int lo = (int)__ldcg(&la.rec->old_ld[i]), ln = (int)__ldcg(&la.rec->new_ld[i]);
-                if (lo < NSL && ((__ldcg(&la.rec->old_row[i][lo >> 5]) >> (lo & 31)) & 1u)) --s_lcnt[lo];
-                if (ln < NSL && ((__ldcg(&la.rec->new_row[i][ln >> 5]) >> (ln & 31)) & 1u)) ++s_lcnt[ln];
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) s_st[j] = __ldcg(&la.rec->state[j]);
-        }
-        __syncthreads();
-        if (s_red[kWarps]) break;
-    }
-}
-
-// The search kernel of a replication session (docs/MODEL.md §11): search_large_kernel with every row's C1 / C7 operands
-// from rftab ([Ppad] packed words, replication_table in kao_host.hpp); kTopicRows 1: with the topic rows of ta, 0:
-// without.  A separate body on purpose: with one force-inlined body shared by both kernels, nvcc schedules the plain
-// kernels differently, and their code is kept exactly as it was (tests/golden/sass_parent_large_engine.json).
-// TWIN of search_large_kernel: it differs only in the two evaluation calls, keep the rest line for line the same.
-template <int W, int kTopicRows>
-__global__ void __launch_bounds__(kLT, 1)
-search_large_rf_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round, uint32_t rounds,
-                       uint32_t round_size, unsigned long long *keys, unsigned int *grid_bar, P2P pp,
-                       unsigned long long *all_keys, TopicArgs ta, const uint32_t *rftab)
-{
-    constexpr bool kTopics = kTopicRows != 0;
-    constexpr int kWarps = kLT / 32, NSL = 32 * W;
-    __shared__ Consts s_cs;
-    __shared__ int s_cnt[256], s_lcnt[256], s_rc[32];
-    __shared__ long long s_acc[2];
-    __shared__ int s_base[3];                          // (violation, objective) of the base; [2] = 1: taken from the last key
-    __shared__ int s_st[4];                            // LargeRecord::state of the current base
-    __shared__ unsigned long long s_red[kWarps + 3];   // per-warp minima; stop flag, best (violation, cost), stall
-    __shared__ int s_abort;
-    __shared__ LargeRecord s_rec;
-    __shared__ ListChanges s_lc;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-    load_consts(&s_cs, d.consts);
-    if (tid < 4) s_st[tid] = __ldcg(d.nD + tid);
-    if (tid == 0) {
-        s_abort = 0; s_base[2] = 0;
-        s_red[kWarps] = 0; s_red[kWarps + 1] = pp.best_in; s_red[kWarps + 2] = pp.stall_in;
-    }
-    __syncthreads();
-    uint32_t barriers = 0;                             // grid barriers passed: two per round with a winner
-    for (uint32_t t = 0; t < rounds; ++t) {
-        const uint32_t round = first_round + t;
-        // the base's own evaluation and totals: a full pass in the first round; afterwards the totals are patched and
-        // the evaluation IS the previous winner's key (unless that key was saturated)
-        if (t == 0 || s_base[2] == 0) {
-            block_eval<W, true>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc, rftab);
-            if constexpr (kTopics) {
-                if (tid == 0) s_acc[0] += __ldcg(ta.tviol);
-            }
-            if (tid == 0) { s_base[0] = (int)min(s_acc[0], (long long)0x7FFFFFFF); s_base[1] = (int)s_acc[1]; }
-            __syncthreads();
-        }
-        unsigned long long best = kKeyNone;
-        {
-            const Gen<W, true, true> tg = large_gen<W>(d, la, &s_cs, s_st);
-            const MemRef<false> m_obj(d.swT);
-            const int base_viol = s_base[0], base_obj = s_base[1];
-            for (uint32_t idx = pp.idx_lo + blockIdx.x * kLT + tid; idx < pp.idx_hi; idx += gridDim.x * kLT) {
-                PatchSet ps;
-                uint32_t rows[kMaxOps][W];
-                tg.run(seed, round, idx, round_size, ps, rows);
-                int viol, obj;
-                delta_eval_rf<W>(d, rftab, m_obj, &s_cs, ps, rows, s_cnt, s_lcnt, s_rc, base_viol, base_obj, viol, obj);
+                delta_eval<LargeCfg<W>, false, kRF>(d, d.bitsT, d.leader, m_obj, &s_cs, ps, rows, s_cnt, s_lcnt, s_rc,
+                                                    base_viol, base_obj, viol, obj, rftab);
                 if constexpr (kTopics) {
                     int rc[2 * kMaxOps], lc[2 * kMaxOps];
                     topic_events<W>(d, ta, &s_cs, ps, rows, rc, lc);
@@ -813,32 +556,18 @@ eval_large_kernel(Params d, const uint32_t *bits, const uint8_t *leader, long lo
     if (threadIdx.x == 0) { viol[a] = s_acc[0]; obj[a] = s_acc[1]; }
 }
 
-// a topic session's base: the evaluation above plus the topic-row violation kept current with the base
-template <int W>
+// the base of a topic or replication session: the evaluation above, with every row's own C1 / C7 operands (kRF), plus
+// the topic-row violation kept current with the base when the session has topic rows (ta.tviol != nullptr)
+template <int W, bool kRF>
 __global__ void __launch_bounds__(kLT, 1)
-eval_large_topics_kernel(Params d, TopicArgs ta, long long *viol, long long *obj)
+eval_large_base_kernel(Params d, TopicArgs ta, const uint32_t *rftab, long long *viol, long long *obj)
 {
     __shared__ Consts s_cs;
     __shared__ int s_cnt[256], s_lcnt[256], s_rc[32];
     __shared__ long long s_acc[2];
     load_consts(&s_cs, d.consts);
     __syncthreads();
-    block_eval<W>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc);
-    if (threadIdx.x == 0) { *viol = s_acc[0] + __ldcg(ta.tviol); *obj = s_acc[1]; }
-}
-
-// a replication session's base: every row with its own C1 / C7 operands, plus the topic-row violation when the
-// session has topic rows (ta.tviol != nullptr)
-template <int W>
-__global__ void __launch_bounds__(kLT, 1)
-eval_large_rf_kernel(Params d, TopicArgs ta, const uint32_t *rftab, long long *viol, long long *obj)
-{
-    __shared__ Consts s_cs;
-    __shared__ int s_cnt[256], s_lcnt[256], s_rc[32];
-    __shared__ long long s_acc[2];
-    load_consts(&s_cs, d.consts);
-    __syncthreads();
-    block_eval<W, true>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc, rftab);
+    block_eval<W, kRF>(d, &s_cs, d.bitsT, d.leader, s_cnt, s_lcnt, s_rc, s_acc, rftab);
     if (threadIdx.x == 0) { *viol = s_acc[0] + (ta.tviol ? __ldcg(ta.tviol) : 0); *obj = s_acc[1]; }
 }
 
@@ -893,29 +622,22 @@ cudaError_t large_search(int W, int grid, const Params &d, const LargeArgs &la, 
     return with_w(W, [&](auto w) {
         constexpr int kW = decltype(w)::value;
         // cooperative launch: all CTAs are co-resident, which the grid barriers need
-        const void *kern = rftab ? (ta ? reinterpret_cast<const void *>(search_large_rf_kernel<kW, 1>)
-                                       : reinterpret_cast<const void *>(search_large_rf_kernel<kW, 0>))
-                                 : (ta ? reinterpret_cast<const void *>(search_large_kernel<kW, true>)
-                                       : reinterpret_cast<const void *>(search_large_kernel<kW, false>));
+        const void *kern = rftab ? (ta ? reinterpret_cast<const void *>(search_large_kernel<kW, true, true>)
+                                       : reinterpret_cast<const void *>(search_large_kernel<kW, false, true>))
+                                 : (ta ? reinterpret_cast<const void *>(search_large_kernel<kW, true, false>)
+                                       : reinterpret_cast<const void *>(search_large_kernel<kW, false, false>));
         return cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kLT), args, 0, st);
     });
 }
 
-cudaError_t large_eval_rf(int W, const Params &d, const TopicArgs *ta, const uint32_t *rftab, long long *viol,
-                          long long *obj, cudaStream_t st)
+cudaError_t large_eval_base(int W, const Params &d, const TopicArgs *ta, const uint32_t *rftab, long long *viol,
+                            long long *obj, cudaStream_t st)
 {
     const TopicArgs t = ta ? *ta : TopicArgs{};
     return with_w(W, [&](auto w) {
-        eval_large_rf_kernel<decltype(w)::value><<<1, kLT, 0, st>>>(d, t, rftab, viol, obj);
-        return cudaGetLastError();
-    });
-}
-
-cudaError_t large_eval_topics(int W, const Params &d, const TopicArgs &ta, long long *viol, long long *obj,
-                              cudaStream_t st)
-{
-    return with_w(W, [&](auto w) {
-        eval_large_topics_kernel<decltype(w)::value><<<1, kLT, 0, st>>>(d, ta, viol, obj);
+        constexpr int kW = decltype(w)::value;
+        if (rftab) eval_large_base_kernel<kW, true><<<1, kLT, 0, st>>>(d, t, rftab, viol, obj);
+        else eval_large_base_kernel<kW, false><<<1, kLT, 0, st>>>(d, t, rftab, viol, obj);
         return cudaGetLastError();
     });
 }

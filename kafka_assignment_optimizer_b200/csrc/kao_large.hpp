@@ -56,12 +56,10 @@ cudaError_t large_search(int W, int grid, const Params &d, const LargeArgs &la, 
                          uint32_t rounds, uint32_t round_size, unsigned long long *keys, unsigned int *grid_bar,
                          const P2P &pp, unsigned long long *all_keys, cudaStream_t st, const TopicArgs *ta = nullptr,
                          const uint32_t *rftab = nullptr);
-// full evaluation of a replication session's base with its per-partition rows (and its topic rows when ta != nullptr)
-cudaError_t large_eval_rf(int W, const Params &d, const TopicArgs *ta, const uint32_t *rftab, long long *viol,
-                          long long *obj, cudaStream_t st);
+// full evaluation of a topic or replication session's base: with its topic rows when ta != nullptr, with its
+// per-partition rows when rftab != nullptr
+cudaError_t large_eval_base(int W, const Params &d, const TopicArgs *ta, const uint32_t *rftab, long long *viol,
+                            long long *obj, cudaStream_t st);
 // full evaluation of n explicit assignments (bits [n][W][Ppad], leaders [n][Ppad]): one CTA each
 cudaError_t large_eval(int W, const Params &d, const uint32_t *bits, const uint8_t *leader, int n, long long *viol,
                        long long *obj, cudaStream_t st);
-// full evaluation of a topic session's base, topic rows included
-cudaError_t large_eval_topics(int W, const Params &d, const TopicArgs &ta, long long *viol, long long *obj,
-                              cudaStream_t st);

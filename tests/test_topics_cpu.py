@@ -178,15 +178,17 @@ def _nvcc():
     return nvcc
 
 
-def test_topic_kernels_do_not_spill():
+def test_topic_instantiations_do_not_spill():
     nvcc = _nvcc()
     with tempfile.TemporaryDirectory() as d:
         out = subprocess.run([nvcc, "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xptxas", "-v",
                               "-Xptxas", "-dlcm=cg", "-c", "-o", os.path.join(d, "k.o"), os.path.join(CSRC, "kao_large.cu")],
                              capture_output=True, text=True, check=True).stderr
     props = re.findall(r"Function properties for (\S+)\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", out)
-    topic = [p for p in props if "ELb1E" in p[0] or "topic" in p[0]]
-    assert len(topic) == 16                                 # search (ELb1E), eval, count and violation kernels, 4 widths
+    topic = [p for p in props if re.search(r"search_large_kernelILi\dELb1E|eval_large_base_kernel|topic_", p[0])]
+    # search (kTopics, with and without per-partition rows), base evaluation (with and without them), count and
+    # violation kernels, 4 widths
+    assert len(topic) == 24
     assert all(p[2] == "0" and p[3] == "0" for p in topic), topic
 
 
@@ -206,9 +208,11 @@ def _sass(obj):
     return res
 
 
-def test_existing_kernels_keep_their_sass():
-    """Every kernel of the large-path and engine objects as the build before the topic rows made it: the plain search
-    kernel is now the kTopics = false instantiation, with TopicArgs appended after every parameter it had."""
+def test_plain_and_topic_kernels_keep_their_pinned_sass():
+    """Every kernel of the large-path and engine objects as the build before the topic rows made it, and the topic search
+    kernels as the build before the per-partition rows made them: the plain search kernel became the kTopics = false
+    instantiation, with TopicArgs appended after every parameter it had, and then every search kernel became the
+    kRF = false instantiation, with the rftab pointer appended."""
     _nvcc()
     pin = json.load(open(os.path.join(ROOT, "tests", "golden", "sass_parent_large_engine.json")))
     for obj, kernels in pin["objects"].items():
@@ -218,6 +222,7 @@ def test_existing_kernels_keep_their_sass():
         now = _sass(path)
         for name, want in kernels.items():
             cur = re.sub(r"search_large_kernelILi(\d)EEEv(.*)$", r"search_large_kernelILi\1ELb0EEEv\g<2>9TopicArgs", name)
+            cur = re.sub(r"search_large_kernelILi(\d)ELb(\d)EEEv(.*)$", r"search_large_kernelILi\1ELb\2ELb0EEEv\g<3>PKj", cur)
             ins = now[cur]
             assert (len(ins), hashlib.sha256("\n".join(ins).encode()).hexdigest()) == (want["instructions"], want["sha256"]), name
 
