@@ -70,8 +70,9 @@ typedef struct kao_problem {
     const int32_t *ldr_hi;    /* [B] C4 max */
     const int32_t *rack_lo;   /* [R] C6 min total replicas per rack, README.md:173-176 */
     const int32_t *rack_hi;   /* [R] C6 max */
-    int32_t ppr_lo;           /* C7 min replicas of one partition in one rack, README.md:178-180 */
-    int32_t ppr_hi;           /* C7 max */
+    int32_t ppr_lo;           /* C7 min replicas of one partition in one rack, README.md:178-180; 0..63: the
+                                 evaluators sum four 8-slot racks' deficits in one byte (4 * 63 = 252) */
+    int32_t ppr_hi;           /* C7 max, ppr_lo..127 */
     const int32_t *cur;       /* [P*RFcur] current assignment, leader first (README.md:52-63),
                                  dense indices; -1 = padding or a broker not in the target list */
 } kao_problem;
@@ -216,8 +217,10 @@ int kao_create_topics(const kao_problem *pb, const kao_topics *tp, int32_t devic
  * pb->RF stays the width of every replica list ([P*RF], -1 padded) and must be >= every rf[p]; pb->ppr_lo / ppr_hi are
  * still validated but not used.  The initial base (MODEL §4) keeps or completes each row to rf[p].  Every other row,
  * the objective, the candidate stream and the key layout stay as they are.  Valid input: 1 <= rf[p] <= min(RF, B - 1),
- * 0 <= ppr_lo[p] <= ppr_hi[p] <= 127, and with topic rows, rep_lo[t] <= the sum of rf over topic t; anything else is
- * KAO_E_ARG before any CUDA call.  The defaults of the Python binding are ppr = floor / ceil of rf[p] / R.
+ * 0 <= ppr_lo[p] <= 63, ppr_lo[p] <= ppr_hi[p] <= 127 (as for pb->ppr_lo / ppr_hi: the evaluators sum the C7 deficits
+ * of four 8-slot racks in one byte, exact up to 4 * 63), and with topic rows, rep_lo[t] <= the sum of rf over topic t;
+ * anything else is KAO_E_ARG before any CUDA call.  The defaults of the Python binding are ppr = floor / ceil of
+ * rf[p] / R.
  */
 typedef struct kao_replication {
     const int32_t *rf;                  /* [P] exactly rf[p] replicas */

@@ -65,7 +65,10 @@ inline bool build_host_model(const kao_problem &pb, HostModel &m, std::string &w
     if (!pb.rack_of || !pb.wF || !pb.wL || !pb.rep_lo || !pb.rep_hi || !pb.ldr_lo || !pb.ldr_hi ||
         !pb.rack_lo || !pb.rack_hi || !pb.cur)
         return bad("null table pointer");
-    if (pb.ppr_lo < 0 || pb.ppr_lo > pb.ppr_hi || pb.ppr_hi > 127) return bad("bad per-partition-per-rack bounds");
+    // ppr_lo <= 63: the general rack form sums the deficits of four 8-slot racks in one byte (row_rack_terms), exact
+    // up to 4 * 63 = 252; ppr_hi <= 127: the field-wise subtraction keeps one sign bit per byte
+    if (pb.ppr_lo < 0 || pb.ppr_lo > 63 || pb.ppr_lo > pb.ppr_hi || pb.ppr_hi > 127)
+        return bad("bad per-partition-per-rack bounds (0 <= ppr_lo <= 63, ppr_lo <= ppr_hi <= 127)");
     m.P = pb.P; m.B = pb.B; m.R = pb.R; m.RF = pb.RF; m.RFcur = pb.RFcur;
     m.ppr_lo = pb.ppr_lo; m.ppr_hi = pb.ppr_hi;
     m.rack_of.assign(pb.rack_of, pb.rack_of + pb.B);
@@ -447,7 +450,7 @@ inline bool build_host_topics(const kao_problem &pb, const kao_topics &tp, int P
 }
 
 // The per-partition C1 / C7 rows of a kao_replication (docs/MODEL.md §11) into m (built by build_host_model):
-// 1 <= rf[p] <= min(RF, B - 1), 0 <= ppr_lo[p] <= ppr_hi[p] <= 127.
+// 1 <= rf[p] <= min(RF, B - 1), 0 <= ppr_lo[p] <= 63, ppr_lo[p] <= ppr_hi[p] <= 127 (the limits of build_host_model).
 inline bool build_host_replication(const kao_replication &rp, HostModel &m, std::string &why)
 {
     auto bad = [&](const std::string &s) { why = "per-partition replication factors: " + s; return false; };
@@ -461,8 +464,9 @@ inline bool build_host_replication(const kao_replication &rp, HostModel &m, std:
         if (f < 1 || f > top)
             return bad("rf[" + std::to_string(p) + "] = " + std::to_string(f) + " is not in 1.." + std::to_string(top) +
                        " (the row width RF, and fewer than the brokers)");
-        if (lo < 0 || lo > hi || hi > 127)
-            return bad("partition " + std::to_string(p) + ": per-rack bounds must satisfy 0 <= ppr_lo <= ppr_hi <= 127");
+        if (lo < 0 || lo > 63 || lo > hi || hi > 127)
+            return bad("partition " + std::to_string(p) +
+                       ": per-rack bounds must satisfy 0 <= ppr_lo <= 63 and ppr_lo <= ppr_hi <= 127");
         m.rf_p[p] = (uint8_t)f; m.ppr_lo_p[p] = (uint8_t)lo; m.ppr_hi_p[p] = (uint8_t)hi;
     }
     return true;

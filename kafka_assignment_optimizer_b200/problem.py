@@ -50,7 +50,9 @@ class Problem:
 @dataclasses.dataclass
 class ReplicationRows:
     """Per-partition replication rows (kao_replication, docs/MODEL.md §11): partition p holds exactly rf[p] replicas,
-    and between ppr_lo[p] and ppr_hi[p] of them in every rack.  They replace the problem's C1 (= RF) and C7."""
+    and between ppr_lo[p] and ppr_hi[p] of them in every rack.  They replace the problem's C1 (= RF) and C7.  The engine
+    accepts 1 <= rf[p] <= min(RF, B - 1), 0 <= ppr_lo[p] <= 63 and ppr_lo[p] <= ppr_hi[p] <= 127: its evaluators sum
+    the C7 deficits of four 8-slot racks in one byte, exact up to 4 * 63."""
     rf: np.ndarray          # int32 [P]
     ppr_lo: np.ndarray      # int32 [P]
     ppr_hi: np.ndarray      # int32 [P]

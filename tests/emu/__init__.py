@@ -25,14 +25,21 @@ def lib():
 
 
 class EmuSession:
-    """Same surface as kafka_assignment_optimizer_b200.Session for the calls the parity tests use."""
+    """Same surface as kafka_assignment_optimizer_b200.Session for the calls the parity tests use.  replication: a
+    ReplicationRows, opened as kao_create_replication does and scored as the HBM-base kernels do (delta keys, whole
+    rounds and get_base only)."""
 
-    def __init__(self, pb):
-        from kafka_assignment_optimizer_b200.optimizer import _CProblem
+    def __init__(self, pb, replication=None):
+        from kafka_assignment_optimizer_b200.optimizer import _CProblem, _CReplication
 
         self.pb = pb
         self._cp = _CProblem(pb)
-        self._h = C.c_void_p(lib().kao_emu_create(self._cp.ref()))
+        self.replication = replication
+        if replication is None:
+            self._h = C.c_void_p(lib().kao_emu_create(self._cp.ref()))
+        else:
+            self._cr = _CReplication(replication)
+            self._h = C.c_void_p(lib().kao_emu_create_replication(self._cp.ref(), self._cr.ref()))
         if not self._h:
             raise ValueError(lib().kao_emu_last_error().decode())
 
@@ -65,6 +72,8 @@ class EmuSession:
         return reps, v.value, o.value, mv.value
 
     def candidate_keys(self, seed, rnd, round_size, idx_begin, count, delta=False):
+        if self.replication is not None and not delta:
+            raise ValueError("a replication session scores candidates by delta evaluation only")
         out = np.empty(count, np.uint64)
         fn = lib().kao_emu_candidate_keys_delta if delta else lib().kao_emu_candidate_keys
         rc = fn(self._h, C.c_uint64(seed), C.c_uint32(rnd), C.c_uint32(round_size), C.c_uint32(idx_begin),
@@ -80,6 +89,8 @@ class EmuSession:
         return keys
 
     def evaluate(self, replicas):
+        if self.replication is not None:
+            raise ValueError("kao_eval scores C1 / C7 against one RF")
         reps = np.ascontiguousarray(replicas, dtype=np.int32)
         n = reps.shape[0]
         v, o = np.empty(n, np.int64), np.empty(n, np.int64)

@@ -4,7 +4,9 @@
 // layout and evaluator configuration exactly as kao_create / dispatch do.  tests/test_device_emulation.py
 // checks it against the committed golden streams and the oracle restatement, so the arithmetic of the
 // CUDA path is exercised by the CPU suite as well; the kernels themselves (staging, grid barrier,
-// cross-GPU exchange) are only tested on the GPU.  Never linked into libkao.so.
+// cross-GPU exchange) are only tested on the GPU.  Replication sessions (kao_emu_create_replication) run the kRF forms
+// of the row and delta evaluators on the HBM-base kernels' configuration (tests/test_replication_emulation.py).
+// Never linked into libkao.so.
 #define KAO_HOST_EMU 1
 #include "warp_emu.hpp"
 
@@ -39,6 +41,10 @@ struct Emu {
     int nW = 0;
     std::vector<uint32_t> T, Z;          // transposed planes, term planes of the objective
     int n_invalid = 0;                   // partitions led from a slot that holds none of their replicas (s_counts[2] of the kernel)
+    // a replication session (kao_create_replication): every row's C1 / C7 operands from rftab, evaluated as the
+    // HBM-base kernels do (kao_large.cu: LargeCfg<W>, block_eval / delta_eval with kRF)
+    bool rf = false;
+    std::vector<uint32_t> rftab;         // [Ppad] rf | ppr_lo << 8 | ppr_hi << 16 (replication_table)
     std::string err;
 };
 
@@ -278,6 +284,151 @@ template <class F> auto dispatch(Emu &e, F f)
     return f(Run<EvalCfg<1, 5, 0, 0>>{});
 }
 
+// The HBM-base kernels of a replication session (kao_large.cu: search_large_kernel<W, false, true>,
+// eval_large_base_kernel<W, true>): their one evaluator configuration, every row's C1 / C7 operands from rftab.
+template <int W> using LargeCfg = EvalCfg<W, 5, 0, kObjEntries>;
+
+template <int W> struct RunRf {
+    struct Totals {
+        std::vector<int> cnt = std::vector<int>(256, 0), lcnt = std::vector<int>(256, 0), rc = std::vector<int>(32, 0);
+        long long viol = 0, obj = 0;                   // raw, as block_eval leaves them in acc
+    };
+    // block_eval<W, true>: row_eval with each row's own operands, the replica / valid-leader count per slot and the
+    // replica count per rack, then the C3 / C4 / C6 bands
+    static Totals base(const Emu &e)
+    {
+        const Params &d = e.prm;
+        const MemRef<false> m_obj(d.swT);
+        Totals t;
+        for (int p = 0; p < d.P; ++p) {
+            uint32_t x[W];
+            for (int w = 0; w < W; ++w) x[w] = e.bits[(size_t)w * d.Ppad + p];
+            const uint32_t ld = e.leader[p];
+            int rv, ro;
+            row_eval<LargeCfg<W>, false, true>(d, m_obj, p, x, ld, rv, ro, row_rf(e.rftab.data(), p));
+            t.viol += rv;
+            t.obj += ro;
+            for (int w = 0; w < W; ++w)
+                for (uint32_t m = x[w]; m; m &= m - 1) {
+                    const int s = 32 * w + __ffs(m) - 1;
+                    ++t.cnt[s];
+                    ++t.rc[s >> d.log2S];
+                }
+            if ((int)ld < 32 * W && row_has<W>(x, (int)ld)) ++t.lcnt[ld];
+        }
+        for (int s = 0; s < 32 * W; ++s)
+            t.viol += band_violation(t.cnt[s], e.cs.bnd_rep[s]) + band_violation(t.lcnt[s], e.cs.bnd_ldr[s]);
+        for (int r = 0; r < d.R; ++r)
+            t.viol += std::max(t.rc[r] - e.cs.rack_hi[r], 0) + std::max(e.cs.rack_lo[r] - t.rc[r], 0);
+        return t;
+    }
+    // the per-thread generator on the base (its linear-scan form), as large_gen hands it to each thread
+    static void gen(const Emu &e, uint64_t seed, uint32_t round, uint32_t idx, uint32_t round_size, PatchSet &ps,
+                    uint32_t (&rows)[kMaxOps][W])
+    {
+        Gen<W, true> tg;
+        tg.bitsT = e.bits.data(); tg.leader = e.leader.data(); tg.cs = &e.cs; tg.d = &e.prm; tg.prow = nullptr; tg.lane = 0;
+        tg.D = e.D.data(); tg.DL = e.DL.data(); tg.nD = e.nD; tg.nL = e.nL;
+        tg.run(seed, round, idx, round_size, ps, rows);
+    }
+    // one candidate of the search kernel: delta_eval<LargeCfg<W>, false, true> on the base's totals
+    static unsigned long long key(const Emu &e, const Totals &t, int base_viol, int base_obj, uint64_t seed,
+                                  uint32_t round, uint32_t idx, uint32_t round_size)
+    {
+        PatchSet ps;
+        uint32_t rows[kMaxOps][W];
+        gen(e, seed, round, idx, round_size, ps, rows);
+        int viol, obj;
+        delta_eval<LargeCfg<W>, false, true>(e.prm, e.bits.data(), e.leader.data(), MemRef<false>(e.prm.swT), &e.cs, ps,
+                                             rows, t.cnt.data(), t.lcnt.data(), t.rc.data(), base_viol, base_obj, viol,
+                                             obj, e.rftab.data());
+        return pack_key(viol, obj, idx, e.prm.key_obj_bits);
+    }
+    // the base's (violation, objective) as the kernel hands it to delta_eval: the full pass, the violation clamped to int
+    static void base_key_fields(const Totals &t, int &bv, int &bo)
+    {
+        bv = (int)std::min(t.viol, (long long)0x7FFFFFFF);
+        bo = (int)t.obj;
+    }
+    static void keys(Emu &e, uint64_t seed, uint32_t round, uint32_t round_size, uint32_t idx_begin, uint32_t count,
+                     uint64_t *out)
+    {
+        const Totals t = base(e);
+        int bv, bo;
+        base_key_fields(t, bv, bo);
+        for (uint32_t i = 0; i < count; ++i) out[i] = key(e, t, bv, bo, seed, round, idx_begin + i, round_size);
+    }
+    // whole rounds as search_large_kernel runs them: after a winner the base's evaluation IS the winner's key, unless
+    // that key is saturated, then the next round evaluates the base in full (the totals are rebuilt here every round,
+    // the kernel patches them: the same counts)
+    static void search(Emu &e, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
+                       uint64_t *round_keys)
+    {
+        bool from_key = false;
+        int bv = 0, bo = 0;
+        for (uint32_t t = 0; t < rounds; ++t) {
+            const uint32_t round = first_round + t;
+            const Totals tot = base(e);
+            if (!from_key) base_key_fields(tot, bv, bo);
+            unsigned long long best = kKeyNone;
+            for (uint32_t idx = 0; idx < round_size; ++idx) best = std::min(best, key(e, tot, bv, bo, seed, round, idx, round_size));
+            if (round_keys) round_keys[t] = best;
+            const uint32_t kv = key_violation(best, e.prm.key_obj_bits);
+            from_key = best != kKeyNone && (uint64_t)kv < key_viol_cap(e.prm.key_obj_bits);
+            bv = (int)kv;
+            bo = (int)key_objective(best, e.prm.key_obj_bits);
+            if (best == kKeyNone) continue;
+            PatchSet win;
+            uint32_t rows[kMaxOps][W];
+            gen(e, seed, round, (uint32_t)(best & kIdxMask), round_size, win, rows);
+            for (int i = 0; i < win.n; ++i) {
+                for (int w = 0; w < W; ++w) e.bits[(size_t)w * e.hm.Ppad + win.p[i]] = rows[i][w];
+                e.leader[win.p[i]] = (uint8_t)win.ld[i];
+            }
+            rebuild_lists(e);
+        }
+    }
+};
+
+template <class F> auto with_w(const Emu &e, F f)
+{
+    switch (e.hm.W) {
+    case 1: return f(RunRf<1>{});
+    case 2: return f(RunRf<2>{});
+    case 4: return f(RunRf<4>{});
+    default: return f(RunRf<8>{});
+    }
+}
+
+// the device-side tables and Params of a session whose host model and evaluator configuration are set; its initial base
+void start(Emu &e)
+{
+    const HostModel &m = e.hm;
+    e.nW = t_words(m.Ppad);
+    fill_consts(m, e.cs);
+    Params &p = e.prm;
+    p.P = m.P; p.Ppad = m.Ppad; p.B = m.B; p.R = m.R; p.RF = m.RF; p.NS = m.NS; p.log2S = m.log2S;
+    set_rf_masks(p);
+    p.key_obj_bits = m.key_obj_bits;
+    p.ppr_lo = m.ppr_lo; p.ppr_hi = m.ppr_hi; p.dense = m.dense ? 1 : 0;
+    p.nentries = m.nentries; p.nplanes = m.nplanes; p.plane_on_leader = m.plane_on_leader;
+    for (int c = 0; c < 6; ++c) p.plane_value[c] = m.plane_value[c];
+    p.swT = m.swT.data();
+    p.planesT = m.nplanes > 0 ? m.planesT.data() : nullptr;
+    p.dense_w = m.dense ? m.dense_w.data() : nullptr;
+    p.homeT = m.homeT.data();
+    p.nz = m.z_ok ? m.nz : 0; p.z_on_leader = m.z_on_leader; p.zslot = m.z_ok ? m.zslot.data() : nullptr;
+    for (int j = 0; j < 8; ++j) p.z_value[j] = m.z_value[j];
+    p.consts = &e.cs;
+    e.D.assign(m.Ppad, 0);
+    e.DL.assign(m.Ppad, 0);
+    e.prow.assign((size_t)kMaxOps * m.W, 0);
+    std::vector<uint32_t> bitsT;
+    std::vector<uint8_t> leader;
+    initial_base(m, bitsT, leader);
+    set_base(e, bitsT, leader);
+}
+
 thread_local std::string g_err;
 
 }  // namespace
@@ -306,29 +457,22 @@ void *kao_emu_create(const kao_problem *pb)
     // kao_set_evaluator: the column-major evaluator covers 8-slot rack fields with C7 = "at most one
     // replica per rack" and an objective of up to eight term planes
     e->trans_ok = m.W <= 2 && m.hi1 && m.log2S == 3 && m.z_ok && column_major_fits(m.W, m.Ppad, 1024, m.P, m.RF);
-    e->nW = t_words(m.Ppad);
-    fill_consts(m, e->cs);
-    Params &p = e->prm;
-    p.P = m.P; p.Ppad = m.Ppad; p.B = m.B; p.R = m.R; p.RF = m.RF; p.NS = m.NS; p.log2S = m.log2S;
-    set_rf_masks(p);
-    p.key_obj_bits = m.key_obj_bits;
-    p.ppr_lo = m.ppr_lo; p.ppr_hi = m.ppr_hi; p.dense = m.dense ? 1 : 0;
-    p.nentries = m.nentries; p.nplanes = m.nplanes; p.plane_on_leader = m.plane_on_leader;
-    for (int c = 0; c < 6; ++c) p.plane_value[c] = m.plane_value[c];
-    p.swT = m.swT.data();
-    p.planesT = m.nplanes > 0 ? m.planesT.data() : nullptr;
-    p.dense_w = m.dense ? m.dense_w.data() : nullptr;
-    p.homeT = m.homeT.data();
-    p.nz = m.z_ok ? m.nz : 0; p.z_on_leader = m.z_on_leader; p.zslot = m.z_ok ? m.zslot.data() : nullptr;
-    for (int j = 0; j < 8; ++j) p.z_value[j] = m.z_value[j];
-    p.consts = &e->cs;
-    e->D.assign(m.Ppad, 0);
-    e->DL.assign(m.Ppad, 0);
-    e->prow.assign((size_t)kMaxOps * m.W, 0);
-    std::vector<uint32_t> bitsT;
-    std::vector<uint8_t> leader;
-    initial_base(m, bitsT, leader);
-    set_base(*e, bitsT, leader);
+    start(*e);
+    return e.release();
+}
+
+// kao_create_replication: the host model with every row's C1 / C7 operands, always on the HBM-base path (no
+// shared-memory plan; objective from packed entries or the dense table; general rack form whatever hi1 says)
+void *kao_emu_create_replication(const kao_problem *pb, const kao_replication *rp)
+{
+    auto e = std::make_unique<Emu>();
+    if (!build_host_model(*pb, e->hm, g_err) || !build_host_replication(*rp, e->hm, g_err)) return nullptr;
+    e->hm.nplanes = 0;
+    e->hm.z_ok = false;
+    e->rf = true;
+    e->rftab = replication_table(e->hm);
+    e->nph = 5; e->rack = 0; e->obj = kObjEntries;
+    start(*e);
     return e.release();
 }
 
@@ -386,6 +530,15 @@ void kao_emu_get_base(void *h, int32_t *replicas, int64_t *violation, int64_t *o
     std::vector<uint32_t> bitsT(e.bits.begin(), e.bits.begin() + (size_t)e.hm.W * e.hm.Ppad);
     decode_replicas(e.hm, bitsT, e.leader, replicas);
     if (moves) *moves = count_moves(e.hm, replicas);
+    if (e.rf) {                                 // eval_large_base_kernel<W, true>: the raw violation
+        with_w(e, [&](auto r) {
+            const auto t = decltype(r)::base(e);
+            if (violation) *violation = t.viol;
+            if (objective) *objective = t.obj;
+            return 0;
+        });
+        return;
+    }
     // idx + 1 == round_size is the identity candidate (docs/MODEL.md §5)
     const unsigned long long k = dispatch(e, [&](auto r) { return decltype(r)::key(e, 0, 0, 1, 2); });
     if (violation) *violation = (int64_t)key_violation(k, e.prm.key_obj_bits);
@@ -406,6 +559,10 @@ void kao_emu_candidate_keys(void *h, uint64_t seed, uint32_t round, uint32_t rou
 void kao_emu_search(void *h, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size, uint64_t *round_keys)
 {
     Emu &e = *static_cast<Emu *>(h);
+    if (e.rf) {
+        with_w(e, [&](auto r) { decltype(r)::search(e, seed, first_round, rounds, round_size, round_keys); return 0; });
+        return;
+    }
     dispatch(e, [&](auto r) {
         for (uint32_t t = 0; t < rounds; ++t) {
             unsigned long long best = kKeyNone;
@@ -422,6 +579,10 @@ int kao_emu_candidate_keys_delta(void *h, uint64_t seed, uint32_t round, uint32_
                                  uint32_t count, uint64_t *keys)
 {
     Emu &e = *static_cast<Emu *>(h);
+    if (e.rf) {
+        with_w(e, [&](auto r) { decltype(r)::keys(e, seed, round, round_size, idx_begin, count, keys); return 0; });
+        return 0;
+    }
     const HostModel &m = e.hm;
     std::vector<int> cnt(256, 0), lcnt(256, 0), rc(32 + 4, 0);
     for (int p = 0; p < m.P; ++p) {

@@ -227,6 +227,59 @@ LARGE_SHAPES = {
 }
 
 
+# ---- per-partition replication rows (docs/MODEL.md §11) ---------------------------------------------------------
+# C7 forms of one row with rf replicas in R racks: (lo, hi)
+C7_FORMS = {
+    "floor_ceil": lambda rf, R, rng: (rf // R, -(-rf // R)),
+    "zero": lambda rf, R, rng: (0, 0),                          # every replica is an excess
+    "exact": lambda rf, R, rng: (rf, rf),                       # all of them in every rack
+    "lo_more_racks": lambda rf, R, rng: (1 + rng.randint(2), 2 + rng.randint(3)),   # with R > rf every row misses
+    "hi_above": lambda rf, R, rng: (0, rf + rng.randint(3)),
+    "hi_127": lambda rf, R, rng: (rng.randint(3), 127),
+    "lo_hi_63": lambda rf, R, rng: (63, 63),                    # the largest lower bound: 4 * 63 deficit in one byte
+}
+
+
+def mixed_rows(pb, seed):
+    """Seeded per-partition rows: every tile of len(C7_FORMS) partitions takes each C7 form once, in an order of its
+    own that never repeats the previous partition's form, with rf = 1, the row width RF (min(RF, B - 1)) or a random
+    factor in between."""
+    from kafka_assignment_optimizer_b200 import ReplicationRows
+
+    rng = np.random.RandomState(seed)
+    top = min(pb.RF, pb.B - 1)
+    forms = list(C7_FORMS.values())
+    order = []
+    while len(order) < pb.P:
+        tile = list(rng.permutation(len(forms)))
+        if order and tile[0] == order[-1]:
+            tile = tile[1:] + tile[:1]
+        order += tile
+    rf = np.array([(1, top, 1 + rng.randint(top))[rng.randint(3)] for _ in range(pb.P)], np.int32)
+    lohi = np.array([forms[order[p]](int(rf[p]), pb.R, rng) for p in range(pb.P)], np.int32)
+    return ReplicationRows(rf, lohi[:, 0].copy(), lohi[:, 1].copy())
+
+
+def off_rf_base(pb, reps, seed):
+    """A base of a replication session (rows of rf[p] replicas) with up to a ninth of the rows made longer (those
+    shorter than RF), a ninth made shorter (those of two or more replicas), by one or two replicas each, and a ninth
+    with their leader moved to another broker"""
+    rng = np.random.RandomState(seed)
+    out = reps.copy()
+    n = max(1, pb.P // 9)
+    k = (out >= 0).sum(1)
+    for p in rng.permutation(np.flatnonzero(k < pb.RF))[:n]:       # longer
+        free = [b for b in rng.permutation(pb.B) if b not in out[p]]
+        for i in range(min(pb.RF - k[p], 1 + rng.randint(2), len(free))):
+            out[p, k[p] + i] = free[i]
+    for p in rng.permutation(np.flatnonzero(k > 1))[:n]:           # shorter
+        out[p, max(1, k[p] - 1 - rng.randint(2)):] = -1
+    for p in rng.choice(pb.P, size=n, replace=False):               # a replica moved
+        free = [b for b in rng.permutation(pb.B) if b not in out[p]]
+        out[p, 0] = free[0]
+    return out
+
+
 def emptied_base(pb, reps, seed):
     """A damaged base with rows emptied (their leader byte stays 0xFF: the partitions led from a slot they do not
     hold), replicas moved to random brokers (duplicates collapse) and rows cut short; the damage scales with P."""

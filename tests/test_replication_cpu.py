@@ -125,10 +125,40 @@ def _bound(pb, rr, replicas=None):
     return out.value
 
 
-@pytest.mark.parametrize("make", [readme_mixed, changed_rf])
-def test_bounds_bracket_the_optimum(make):
-    pb = make()
+def seeded_mixed(seed, racks, topics, removed=0):
+    """Brokers 0.. in racks of the given sizes (interleaved), the last `removed` of them leaving; topics: (partitions,
+    rf) pairs, each partition on rf random brokers; every topic keeps its RF (build_problem(keep_rf=True))."""
+    rng = np.random.RandomState(seed)
+    rack = [r for i in range(max(racks)) for r in range(len(racks)) if i < racks[r]]
+    B = len(rack)
+    rows, labels = [], []
+    for t, (n, rf) in enumerate(topics):
+        rows += [[int(b) for b in rng.choice(B, size=rf, replace=False)] for _ in range(n)]
+        labels += [("t%d" % t, q) for q in range(n)]
+    return kao.build_problem(rows, range(B - removed), {b: "r%d" % rack[b] for b in range(B)}, None, labels,
+                             keep_rf=True)
+
+
+BOUND_INSTANCES = {
+    "readme_mixed": readme_mixed,
+    "changed_rf": changed_rf,
+    "lo_above_0": lambda: seeded_mixed(1, [3, 3], [(4, 3), (3, 2), (2, 1)]),         # two racks: C7 1..2 / 1..1
+    "one_rack": lambda: seeded_mixed(2, [5], [(3, 3), (4, 1), (2, 2)]),               # C7 lo = hi = rf[p]
+    "rf1_partitions": lambda: seeded_mixed(3, [3, 3, 3], [(6, 1), (4, 3)], removed=1),
+    "rf_b_minus_1": lambda: seeded_mixed(4, [2, 2], [(3, 3), (3, 1)]),                # four brokers, rf 3
+    "three_factors": lambda: seeded_mixed(5, [3, 3, 2], [(3, 3), (4, 2), (3, 1)], removed=1),
+    "unequal_racks": lambda: seeded_mixed(6, [4, 2, 3], [(5, 2), (3, 3), (2, 1)]),
+}
+
+
+@pytest.mark.parametrize("name", sorted(BOUND_INSTANCES))
+def test_bounds_bracket_the_optimum(name):
+    """kao_solve_replication certifies optimality when a result reaches the cheap bound: both bounds must lie at or
+    above the HiGHS optimum on every instance"""
+    pb = BOUND_INSTANCES[name]()
+    assert pb.replication is not None
     sol = rf_ref.solve_exact(pb, pb.replication)
+    assert sol.status == "optimal", sol.status
     cheap = _bound(pb, pb.replication)
     flow = _bound(pb, pb.replication, sol.replicas)
     assert sol.objective <= flow <= cheap
@@ -168,9 +198,23 @@ def test_invalid_replication_rows_are_refused_without_a_gpu():
            dataclasses.replace(rr, ppr_lo=np.where(np.arange(n) == 4, 2, rr.ppr_lo).astype(np.int32)),  # lo > hi
            dataclasses.replace(rr, ppr_hi=np.full(n, 128, np.int32)),                                 # hi > 127
            dataclasses.replace(rr, ppr_lo=np.full(n, -1, np.int32))]
+    # lo > 63: four 8-slot racks' deficits would wrap the byte they are summed in (docs/MODEL.md §1)
+    for lo in (64, 127):
+        bad.append(dataclasses.replace(rr, ppr_lo=np.where(np.arange(n) == 4, lo, rr.ppr_lo).astype(np.int32),
+                                       ppr_hi=np.where(np.arange(n) == 4, 127, rr.ppr_hi).astype(np.int32)))
     for r in bad:
         for rc, msg in calls(r):
             assert rc == -1 and msg.startswith("per-partition replication factors:"), (rc, msg)
+    # the same limit on the problem's own C7, with and without per-partition rows
+    h = C.c_void_p()
+    for lo in (64, 127):
+        cpl = kopt._CProblem(dataclasses.replace(pb, ppr_lo=lo, ppr_hi=127))
+        rcs = [lib.kao_create(cpl.ref(), C.c_int32(0), C.byref(h)),
+               lib.kao_create_replication(cpl.ref(), None, kopt._CReplication(rr).ref(), C.c_int32(0), C.byref(h))]
+        msg = lib.kao_last_error().decode()
+        assert rcs == [-1, -1] and msg.startswith("bad per-partition-per-rack bounds"), (rcs, msg)
+    cpl = kopt._CProblem(dataclasses.replace(pb, ppr_lo=63, ppr_hi=127))
+    assert lib.kao_key_obj_bits(cpl.ref()) > 0
     # a topic row whose lo exceeds the sum of its partitions' factors (b1: 3 replicas)
     t = dataclasses.replace(tr, rep_lo=np.array([0, 0, 4], np.int32), rep_hi=np.array([9, 9, 9], np.int32))
     for rc, msg in calls(rr, t):
