@@ -244,7 +244,7 @@ def replica_moves(pb: Problem, replicas: np.ndarray) -> int:
     moves = 0
     for p in range(pb.P):
         have = {int(b) for b in pb.cur[p] if b >= 0}
-        moves += sum(1 for b in replicas[p] if int(b) not in have)
+        moves += sum(1 for b in replicas[p] if b >= 0 and int(b) not in have)     # -1 pads a short row
     return moves
 
 

@@ -88,6 +88,14 @@ class EmuSession:
                              C.c_uint32(round_size), C.c_void_p(keys.ctypes.data))
         return keys
 
+    def check_state(self):
+        """The state the walk patched (transposed / term planes, one-hot plane, count of invalid leaders, displaced
+        lists) against the same state rebuilt from the base (kao_emu_check_state) -> (0, -1, "") or (code, index,
+        message)."""
+        at = C.c_int64(-1)
+        rc = lib().kao_emu_check_state(self._h, C.byref(at))
+        return rc, at.value, lib().kao_emu_last_error().decode() if rc else ""
+
     def evaluate(self, replicas):
         if self.replication is not None:
             raise ValueError("kao_eval scores C1 / C7 against one RF")

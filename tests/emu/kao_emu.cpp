@@ -65,17 +65,34 @@ template <int W> void build_T(Emu &e)
 
 uint32_t oh_word(uint32_t x, uint32_t ld, int w) { return ((int)(ld >> 5) == w) ? (x & (1u << (ld & 31u))) : 0u; }
 
+// partitions led from a slot that holds none of their replicas, counted over the whole base (the kernel's staging pass)
+int count_invalid(const Emu &e)
+{
+    const HostModel &m = e.hm;
+    int n = 0;
+    for (int p = 0; p < m.P; ++p) {
+        const int ld = e.leader[p];
+        if (!(ld < 32 * m.W && ((e.bits[(size_t)(ld >> 5) * m.Ppad + p] >> (ld & 31)) & 1u))) ++n;
+    }
+    return n;
+}
+
+// s_counts[2] after a winner's row i replaces partition p's row and leader, as search_persistent_kernel updates it
+// (before the row is written): -1 if the old leader was invalid, +1 if the new one is
+void patch_invalid(Emu &e, int p, const uint32_t *newrow, int ln)
+{
+    const int W = e.hm.W, lo = e.leader[p];
+    const bool was = lo < W * 32 && ((e.bits[(size_t)(lo >> 5) * e.hm.Ppad + p] >> (lo & 31)) & 1u);
+    const bool is = ln < W * 32 && ((newrow[ln >> 5] >> (ln & 31)) & 1u);
+    e.n_invalid += (was ? 0 : -1) + (is ? 0 : 1);
+}
+
 // rebuild_lists of kao_kernels.cuh: ascending partitions that miss a home slot (D) / hold home slot
 // 0 without being led from it (DL)
 void rebuild_lists(Emu &e)
 {
     const HostModel &m = e.hm;
     e.nD = e.nL = 0;
-    e.n_invalid = 0;
-    for (int p = 0; p < m.P; ++p) {
-        const int ld = e.leader[p];
-        if (!(ld < 32 * m.W && ((e.bits[(size_t)(ld >> 5) * m.Ppad + p] >> (ld & 31)) & 1u))) ++e.n_invalid;
-    }
     for (int p = 0; p < m.P; ++p) {
         const uint32_t h4 = m.homeT[p];
         bool miss = false, ldis = false;
@@ -104,7 +121,61 @@ void set_base(Emu &e, const std::vector<uint32_t> &bitsT, const std::vector<uint
     e.prm.bitsT = e.bits.data();
     e.prm.leader = e.leader.data();
     rebuild_lists(e);
+    e.n_invalid = count_invalid(e);
     if (e.trans_ok) { if (m.W == 1) build_T<1>(e); else build_T<2>(e); }
+}
+
+// State a search patches winner by winner, against the same state rebuilt from the current bits / leader: the one-hot
+// plane, the count of invalid leaders, the displaced lists.  0, or 3.. (kao_emu_check_state) with the first differing
+// index in *at and a message in g_err.
+int check_state_msg(int code, const char *what, long long at, long long *out_at, std::string &err)
+{
+    *out_at = at;
+    err = std::string("patched ") + what + " differs from the rebuilt one at index " + std::to_string(at);
+    return code;
+}
+
+int check_base_state(Emu &e, long long *at, std::string &err)
+{
+    const HostModel &m = e.hm;
+    if (e.oh)
+        for (int w = 0; w < m.W; ++w)
+            for (int p = 0; p < m.Ppad; ++p) {
+                const size_t i = (size_t)(m.W + w) * m.Ppad + p;
+                if (e.bits[i] != oh_word(e.bits[(size_t)w * m.Ppad + p], e.leader[p], w))
+                    return check_state_msg(3, "leader one-hot plane", (long long)i, at, err);
+            }
+    const int n_inv = count_invalid(e);
+    if (n_inv != e.n_invalid) {
+        *at = e.n_invalid;
+        err = "patched count of invalid leaders " + std::to_string(e.n_invalid) + ", rebuilt " + std::to_string(n_inv);
+        return 4;
+    }
+    const std::vector<uint16_t> D = e.D, DL = e.DL;
+    const int nD = e.nD, nL = e.nL;
+    rebuild_lists(e);
+    int rc = 0;
+    if (nD != e.nD || nL != e.nL) {
+        *at = nD != e.nD ? 0 : 1;
+        err = "patched list lengths (" + std::to_string(nD) + ", " + std::to_string(nL) + "), rebuilt (" +
+              std::to_string(e.nD) + ", " + std::to_string(e.nL) + ")";
+        rc = 5;
+    }
+    for (int i = 0; rc == 0 && i < nD; ++i)
+        if (D[i] != e.D[i]) rc = check_state_msg(6, "list D", i, at, err);
+    for (int i = 0; rc == 0 && i < nL; ++i)
+        if (DL[i] != e.DL[i]) rc = check_state_msg(7, "list DL", i, at, err);
+    e.D = D; e.DL = DL; e.nD = nD; e.nL = nL;        // the session keeps the state it patched
+    return rc;
+}
+
+// the first index at which two plane arrays differ, or -1
+long long first_diff(const std::vector<uint32_t> &a, const std::vector<uint32_t> &b)
+{
+    if (a.size() != b.size()) return (long long)std::min(a.size(), b.size());
+    for (size_t i = 0; i < a.size(); ++i)
+        if (a[i] != b[i]) return (long long)i;
+    return -1;
 }
 
 template <class Cfg> struct Run {
@@ -210,6 +281,7 @@ template <class Cfg> struct Run {
                         t_patch_row<W>(e.prm, e.T.data(), e.Z.data(), e.nW, win.p[i], newrow, win.ld[i], lane);
                 }
             }
+            patch_invalid(e, win.p[i], &e.prow[(size_t)i * W], win.ld[i]);
             for (int w = 0; w < W; ++w) {
                 const uint32_t v = e.prow[i * W + w];
                 e.bits[(size_t)w * Ppad + win.p[i]] = v;
@@ -609,6 +681,30 @@ int kao_emu_candidate_keys_delta(void *h, uint64_t seed, uint32_t round, uint32_
         return 0;
     });
     return 0;
+}
+
+// The state a search patches winner by winner (transposed and term planes with t_patch_row, the one-hot plane, the
+// count of invalid leaders that decides t_leaders_valid, the displaced lists) against the same state rebuilt from the
+// current bits / leader with the builders set_base uses.  0: equal; else the first array that differs (1 transposed
+// planes, 2 term / rack-field planes, 3 one-hot plane, 4 count of invalid leaders, 5 list lengths, 6 D, 7 DL), its
+// index in *at, a message in kao_emu_last_error.  The session keeps its patched state either way.
+int kao_emu_check_state(void *h, int64_t *at)
+{
+    Emu &e = *static_cast<Emu *>(h);
+    long long i = -1;
+    int rc = 0;
+    if (e.trans_ok && !e.rf) {
+        std::vector<uint32_t> T = e.T, Z = e.Z;
+        if (e.hm.W == 1) build_T<1>(e); else build_T<2>(e);
+        const long long dt = first_diff(T, e.T), dz = first_diff(Z, e.Z);
+        e.T.swap(T);
+        e.Z.swap(Z);
+        if (dt >= 0) rc = check_state_msg(1, "transposed planes", dt, &i, g_err);
+        else if (dz >= 0) rc = check_state_msg(2, "term / rack-field planes", dz, &i, g_err);
+    }
+    if (rc == 0) rc = check_base_state(e, &i, g_err);
+    *at = i;
+    return rc;
 }
 
 // explicit candidates (kao_eval / eval_batch_kernel): replicas [n][P*RF]

@@ -57,6 +57,13 @@ class MmaSession:
                                          C.c_uint32(idx_begin), C.c_uint32(count), C.c_void_p(out.ctypes.data))
         return out
 
+    def check_state(self):
+        """Patched planes, one-hot plane, count of invalid leaders and displaced lists against the same state rebuilt
+        from the base (kao_emu_mma_check_state) -> (0, -1, "") or (code, index, message)."""
+        at = C.c_int64(-1)
+        rc = lib().kao_emu_mma_check_state(self._h, C.byref(at))
+        return rc, at.value, lib().kao_emu_last_error().decode() if rc else ""
+
     def search(self, seed, first_round, rounds, round_size):
         keys = np.zeros(rounds, np.uint64)
         lib().kao_emu_mma_search(self._h, C.c_uint64(seed), C.c_uint32(first_round), C.c_uint32(rounds),

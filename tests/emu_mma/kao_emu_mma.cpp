@@ -100,6 +100,7 @@ template <int W> void apply(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t i
     for (int i = 0; i < win.n; ++i) {
         for (int lane = 0; lane < 32; ++lane)
             t_patch_row<W, true>(e.prm, x.T.data(), x.Z.data(), e.nW, win.p[i], wrows[i], win.ld[i], lane);
+        patch_invalid(e, win.p[i], wrows[i], win.ld[i]);
         for (int w = 0; w < W; ++w) {
             e.bits[(size_t)w * Ppad + win.p[i]] = wrows[i][w];
             if (e.oh) e.bits[(size_t)(W + w) * Ppad + win.p[i]] = oh_word(wrows[i][w], win.ld[i], w);
@@ -159,6 +160,26 @@ void kao_emu_mma_candidate_keys(void *h, uint64_t seed, uint32_t round, uint32_t
         keys<decltype(w)::value>(x, seed, round, idx_begin, count, round_size, reinterpret_cast<unsigned long long *>(out));
         return 0;
     });
+}
+
+// kao_emu_check_state for this session's planes: the transposed, term, rack-field and shortfall planes t_patch_row
+// patched against build_planes on the current base (1 transposed, 2 the others), then the one-hot plane, the count
+// of invalid leaders and the displaced lists (3..7)
+int kao_emu_mma_check_state(void *h, int64_t *at)
+{
+    auto &x = *static_cast<MmaEmu *>(h);
+    long long i = -1;
+    int rc = 0;
+    std::vector<uint32_t> T = x.T, Z = x.Z;
+    with_w(x, [&](auto w) { build_planes<decltype(w)::value>(x); return 0; });
+    const long long dt = first_diff(T, x.T), dz = first_diff(Z, x.Z);
+    x.T.swap(T);
+    x.Z.swap(Z);
+    if (dt >= 0) rc = check_state_msg(1, "transposed planes", dt, &i, g_err);
+    else if (dz >= 0) rc = check_state_msg(2, "term / rack-field / shortfall planes", dz, &i, g_err);
+    if (rc == 0) rc = check_base_state(*x.e, &i, g_err);
+    *at = i;
+    return rc;
 }
 
 // whole rounds: argmin of the keys, the winner becomes the base (kao_search, one GPU, no early stop)
