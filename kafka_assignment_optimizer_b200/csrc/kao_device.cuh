@@ -37,7 +37,7 @@ struct Consts {
     int32_t rack_lo[32];         // C6
     int32_t rack_hi[32];
     uint8_t slot_of_order[256];  // rack-major order index -> slot
-    uint8_t order_of_slot[256];  // slot -> order index, 0xFF for padding slots
+    uint8_t order_of_slot[256];  // slot -> order index, 0xFF for padding slots (slot 255's own index when B = 256)
 };
 static_assert(sizeof(Consts) % 16 == 0, "bulk copy size");
 

@@ -322,8 +322,9 @@ inline void initial_base(const HostModel &m, std::vector<uint32_t> &bitsT, std::
             }
             pl.set(p, m.slot_of_broker[best]);
             ++load[best];
-            ++count[p];
-            if (leader[p] == 0xFF) leader[p] = (uint8_t)m.slot_of_broker[best];
+            // a row without survivors is led from its first added replica (the leader byte cannot say "not led yet":
+            // 0xFF is slot 255 when every slot holds a broker)
+            if (count[p]++ == 0) leader[p] = (uint8_t)m.slot_of_broker[best];
         }
     }
 }

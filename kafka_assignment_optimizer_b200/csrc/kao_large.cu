@@ -109,76 +109,6 @@ __device__ __forceinline__ void displaced(uint32_t h4, const uint32_t (&row)[W],
     }
 }
 
-__device__ __forceinline__ int band_int(int c, int lo, int hi) { return max(c - hi, 0) + max(lo - c, 0); }
-
-// The topic events of a candidate (docs/MODEL.md §10): a patched row differs from the base by at most one replica
-// move and one leader change, so it gives at most one -1 / +1 replica event and one -1 / +1 valid-leader event, each on
-// the cell topic * 32 W + slot.  Padding slots carry no topic row: -1 (no event) there.
-// Events of patched row i (partition p, leader ldo -> ldn, words old_word(w) -> new_word(w)) into entries 2 i, 2 i + 1.
-template <int W, class Old, class New>
-__device__ __forceinline__ void topic_row_events(const TopicArgs &ta, const Consts *cs, int i, int p, int ldo, int ldn,
-                                                 Old old_word, New new_word, int (&rc)[2 * kMaxOps],
-                                                 int (&lc)[2 * kMaxOps])
-{
-    constexpr int NSL = 32 * W;
-    auto cell = [&](int t, int s) { return (s >= 0 && cs->order_of_slot[s] != 0xFF) ? t * NSL + s : -1; };
-    const int t = ta.topic_of[p];
-    // one word at a time (no row copies: the W = 8 kernel has no registers to spare)
-    int rs = -1, as = -1;
-    bool oko = false, okn = false;
-#pragma unroll
-    for (int w = 0; w < W; ++w) {
-        const uint32_t o = old_word(w), n = new_word(w);
-        if (o & ~n) rs = 32 * w + __ffs(o & ~n) - 1;
-        if (n & ~o) as = 32 * w + __ffs(n & ~o) - 1;
-        if ((ldo >> 5) == w) oko = (o >> (ldo & 31)) & 1u;
-        if ((ldn >> 5) == w) okn = (n >> (ldn & 31)) & 1u;
-    }
-    rc[2 * i] = cell(t, rs);
-    rc[2 * i + 1] = cell(t, as);
-    lc[2 * i] = cell(t, oko ? ldo : -1);
-    lc[2 * i + 1] = cell(t, okn ? ldn : -1);
-}
-
-// the events of a candidate against the base: entry 2 i is row i's -1 event, 2 i + 1 its +1 event (-1: none)
-template <int W>
-__device__ __forceinline__ void topic_events(const Params &d, const TopicArgs &ta, const Consts *cs, const PatchSet &ps,
-                                             const uint32_t (&rows)[kMaxOps][W], int (&rc)[2 * kMaxOps],
-                                             int (&lc)[2 * kMaxOps])
-{
-#pragma unroll
-    for (int i = 0; i < kMaxOps; ++i) {
-        rc[2 * i] = rc[2 * i + 1] = lc[2 * i] = lc[2 * i + 1] = -1;
-        if (i < ps.n) {
-            const int p = ps.p[i];
-            topic_row_events<W>(ta, cs, i, p, d.leader[p], (int)ps.ld[i],
-                                [&](int w) { return d.bitsT[(size_t)w * d.Ppad + p]; },
-                                [&](int w) { return rows[i][w]; }, rc, lc);
-        }
-    }
-}
-
-// change of the topic-row violation from the base to the candidate: the events netted per cell, <= 12 counts read
-template <int W>
-__device__ __forceinline__ int topic_delta(const TopicArgs &ta, const int (&rc)[2 * kMaxOps], const int (&lc)[2 * kMaxOps])
-{
-    constexpr int LOG2_NSL = W == 1 ? 5 : W == 2 ? 6 : W == 4 ? 7 : 8;
-    int val[2 * kMaxOps];
-#pragma unroll
-    for (int j = 0; j < 2 * kMaxOps; ++j) val[j] = (j & 1) ? 1 : -1;
-    int dv = apply_events<2 * kMaxOps>(rc, val, [&](int c, int net) {
-        const int4 b = __ldg(ta.bnd + (c >> LOG2_NSL));
-        const int n = ta.tcnt[c];
-        return band_int(n + net, b.x, b.y) - band_int(n, b.x, b.y);
-    });
-    dv += apply_events<2 * kMaxOps>(lc, val, [&](int c, int net) {
-        const int4 b = __ldg(ta.bnd + (c >> LOG2_NSL));
-        const int n = ta.tlcnt[c];
-        return band_int(n + net, b.z, b.w) - band_int(n, b.z, b.w);
-    });
-    return dv;
-}
-
 // List changes of one round: at most kMaxOps removals and insertions per list
 struct ListChanges {
     int nd[2], ni[2];
@@ -297,24 +227,18 @@ __device__ void apply_winner_large(const Params &d, const LargeArgs &la, const C
 // CTA 0, the thread that wrote the winner record (apply_winner_large): the topic counts and the topic-row violation of
 // the base follow the record's old and new rows
 template <int W>
-__device__ __forceinline__ void apply_winner_topics(const TopicArgs &ta, const Consts *cs, const LargeRecord &rec)
+__device__ __forceinline__ void apply_winner_topics(const TopicArgs &ta, const Consts *cs, int B, const LargeRecord &rec)
 {
     int rc[2 * kMaxOps], lc[2 * kMaxOps];
 #pragma unroll
     for (int i = 0; i < kMaxOps; ++i) {
         rc[2 * i] = rc[2 * i + 1] = lc[2 * i] = lc[2 * i + 1] = -1;
         if (i < rec.n)
-            topic_row_events<W>(ta, cs, i, rec.p[i], (int)rec.old_ld[i], (int)rec.new_ld[i],
+            topic_row_events<W>(ta, cs, B, i, rec.p[i], (int)rec.old_ld[i], (int)rec.new_ld[i],
                                 [&](int w) { return rec.old_row[i][w]; }, [&](int w) { return rec.new_row[i][w]; },
                                 rc, lc);
     }
-    *ta.tviol += topic_delta<W>(ta, rc, lc);
-#pragma unroll
-    for (int j = 0; j < 2 * kMaxOps; ++j) {
-        const int v = (j & 1) ? 1 : -1;
-        if (rc[j] >= 0) ta.tcnt[rc[j]] = (uint16_t)(ta.tcnt[rc[j]] + v);
-        if (lc[j] >= 0) ta.tlcnt[lc[j]] = (uint16_t)(ta.tlcnt[lc[j]] + v);
-    }
+    topic_apply_events<W>(ta, rc, lc);
 }
 
 // the search kernel; kTopics: the topic rows of ta are part of the violation; kRF: every row's C1 / C7 operands from
@@ -427,7 +351,7 @@ search_large_kernel(Params d, LargeArgs la, uint64_t seed, uint32_t first_round,
         }
         if (blockIdx.x == 0) apply_winner_large<W>(d, la, &s_cs, s_st, seed, round, round_size, k, s_rec, s_lc);
         if constexpr (kTopics) {
-            if (blockIdx.x == 0 && tid == 0) apply_winner_topics<W>(ta, &s_cs, s_rec);
+            if (blockIdx.x == 0 && tid == 0) apply_winner_topics<W>(ta, &s_cs, d.B, s_rec);
         }
         // grid barrier 2: the patched HBM state and the winner record are visible before anyone reads them
         __syncthreads();
@@ -484,9 +408,9 @@ __global__ void topic_count_kernel(Params d, TopicArgs ta)
         for (int w = 0; w < W; ++w)
             for (uint32_t m = x[w]; m; m &= m - 1) {
                 const int s = 32 * w + __ffs(m) - 1;
-                if (d.consts->order_of_slot[s] != 0xFF) bump(ta.tcnt, s);
+                if (broker_slot(d.consts, d.B, s)) bump(ta.tcnt, s);
             }
-        if (ld < NSL && row_has<W>(x, ld) && d.consts->order_of_slot[ld] != 0xFF) bump(ta.tlcnt, ld);
+        if (ld < NSL && row_has<W>(x, ld) && broker_slot(d.consts, d.B, ld)) bump(ta.tlcnt, ld);
     }
 }
 
@@ -501,7 +425,7 @@ __global__ void topic_violation_kernel(Params d, TopicArgs ta)
     int v = 0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)ta.T * NSL; i += (size_t)gridDim.x * blockDim.x) {
         const int s = (int)(i & (NSL - 1));
-        if (d.consts->order_of_slot[s] == 0xFF) continue;
+        if (!broker_slot(d.consts, d.B, s)) continue;
         const int4 b = ta.bnd[i / NSL];
         v += band_int(ta.tcnt[i], b.x, b.y) + band_int(ta.tlcnt[i], b.z, b.w);
     }

@@ -3,6 +3,7 @@
 // with delta evaluation only.  Everything else of the engine (kao_engine.cu) stays as it is below that size.
 #pragma once
 #include "kao_kernels.cuh"
+#include "kao_topics.cuh"
 
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -30,17 +31,6 @@ struct LargeArgs {
     uint32_t *T;
     int tnW;
     LargeRecord *rec;
-};
-
-// Per-topic balance rows of a topic session (docs/MODEL.md §10, DESIGN.md §7.2), all in HBM.  The counts are those of
-// the base over broker slots (padding slots are never counted nor read); CTA 0 patches them and tviol from each
-// round's winner before the second grid barrier.
-struct TopicArgs {
-    int T;
-    const uint16_t *topic_of;       // [Ppad] topic of each partition
-    const int4 *bnd;                // [T] (C3t lo, C3t hi, C4t lo, C4t hi)
-    uint16_t *tcnt, *tlcnt;         // [T][32 W] replicas / valid leaders of each topic per slot
-    int *tviol;                     // the base's violation of the topic rows
 };
 
 // the HBM state derived from the base (transposed planes, displaced lists in buffer 0, leader validity count) after

@@ -264,8 +264,10 @@ void kao_ref_init_base(const ref_problem *pb, uint32_t *bits, uint8_t *leader)
                 int ra = pr[pb->rack_of[b]], rb = pr[pb->rack_of[best]];
                 if (ra < rb || (ra == rb && load[b] < load[best])) best = b;
             }
+            /* a row without survivors is led from its first added replica (not "leader byte 0xFF": that is slot
+             * 255 when every slot holds a broker) */
+            if (n == 0) leader[p] = (uint8_t)L.slot_of_broker[best];
             row_set(row, L.slot_of_broker[best]); ++load[best]; ++n;
-            if (leader[p] == 0xFF) leader[p] = (uint8_t)L.slot_of_broker[best];
         }
     }
 }

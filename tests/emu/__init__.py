@@ -19,6 +19,8 @@ def lib():
         subprocess.check_call(["make", "-s", "-C", _HERE])
         _lib = C.CDLL(_SO)
         _lib.kao_emu_create.restype = C.c_void_p
+        _lib.kao_emu_create_replication.restype = C.c_void_p
+        _lib.kao_emu_create_topics.restype = C.c_void_p
         _lib.kao_emu_last_error.restype = C.c_char_p
         _lib.kao_emu_rows_charged_one_by_one.restype = C.c_longlong
     return _lib
@@ -26,20 +28,24 @@ def lib():
 
 class EmuSession:
     """Same surface as kafka_assignment_optimizer_b200.Session for the calls the parity tests use.  replication: a
-    ReplicationRows, opened as kao_create_replication does and scored as the HBM-base kernels do (delta keys, whole
-    rounds and get_base only)."""
+    ReplicationRows, opened as kao_create_replication does; topics: a TopicRows, opened as kao_create_topics does.  Both
+    are scored as the HBM-base kernels do (delta keys, whole rounds and get_base only)."""
 
-    def __init__(self, pb, replication=None):
-        from kafka_assignment_optimizer_b200.optimizer import _CProblem, _CReplication
+    def __init__(self, pb, replication=None, topics=None):
+        from kafka_assignment_optimizer_b200.optimizer import _CProblem, _CReplication, _CTopics
 
+        assert replication is None or topics is None
         self.pb = pb
         self._cp = _CProblem(pb)
-        self.replication = replication
-        if replication is None:
-            self._h = C.c_void_p(lib().kao_emu_create(self._cp.ref()))
-        else:
+        self.large = replication is not None or topics is not None     # the HBM-base kernels' session
+        if replication is not None:
             self._cr = _CReplication(replication)
             self._h = C.c_void_p(lib().kao_emu_create_replication(self._cp.ref(), self._cr.ref()))
+        elif topics is not None:
+            self._ct = _CTopics(topics)
+            self._h = C.c_void_p(lib().kao_emu_create_topics(self._cp.ref(), self._ct.ref()))
+        else:
+            self._h = C.c_void_p(lib().kao_emu_create(self._cp.ref()))
         if not self._h:
             raise ValueError(lib().kao_emu_last_error().decode())
 
@@ -72,8 +78,8 @@ class EmuSession:
         return reps, v.value, o.value, mv.value
 
     def candidate_keys(self, seed, rnd, round_size, idx_begin, count, delta=False):
-        if self.replication is not None and not delta:
-            raise ValueError("a replication session scores candidates by delta evaluation only")
+        if self.large and not delta:
+            raise ValueError("a replication or topic session scores candidates by delta evaluation only")
         out = np.empty(count, np.uint64)
         fn = lib().kao_emu_candidate_keys_delta if delta else lib().kao_emu_candidate_keys
         rc = fn(self._h, C.c_uint64(seed), C.c_uint32(rnd), C.c_uint32(round_size), C.c_uint32(idx_begin),
@@ -97,8 +103,8 @@ class EmuSession:
         return rc, at.value, lib().kao_emu_last_error().decode() if rc else ""
 
     def evaluate(self, replicas):
-        if self.replication is not None:
-            raise ValueError("kao_eval scores C1 / C7 against one RF")
+        if self.large:
+            raise ValueError("kao_eval scores C1 / C7 against one RF and without topic rows")
         reps = np.ascontiguousarray(replicas, dtype=np.int32)
         n = reps.shape[0]
         v, o = np.empty(n, np.int64), np.empty(n, np.int64)

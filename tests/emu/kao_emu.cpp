@@ -5,13 +5,15 @@
 // checks it against the committed golden streams and the oracle restatement, so the arithmetic of the
 // CUDA path is exercised by the CPU suite as well; the kernels themselves (staging, grid barrier,
 // cross-GPU exchange) are only tested on the GPU.  Replication sessions (kao_emu_create_replication) run the kRF forms
-// of the row and delta evaluators on the HBM-base kernels' configuration (tests/test_replication_emulation.py).
+// of the row and delta evaluators on the HBM-base kernels' configuration (tests/test_replication_emulation.py); topic
+// sessions (kao_emu_create_topics) add the topic rows of csrc/kao_topics.cuh to it (tests/test_slot255_cpu.py).
 // Never linked into libkao.so.
 #define KAO_HOST_EMU 1
 #include "warp_emu.hpp"
 
 #include "../../kafka_assignment_optimizer_b200/csrc/kao_device.cuh"
 #include "../../kafka_assignment_optimizer_b200/csrc/kao_device_t.cuh"
+#include "../../kafka_assignment_optimizer_b200/csrc/kao_topics.cuh"
 #include "../../kafka_assignment_optimizer_b200/csrc/kao_plan.hpp"
 #include "../../kafka_assignment_optimizer_b200/csrc/kao_host.hpp"
 
@@ -45,6 +47,14 @@ struct Emu {
     // HBM-base kernels do (kao_large.cu: LargeCfg<W>, block_eval / delta_eval with kRF)
     bool rf = false;
     std::vector<uint32_t> rftab;         // [Ppad] rf | ppr_lo << 8 | ppr_hi << 16 (replication_table)
+    // a topic session (kao_create_topics): the same kernels with the topic rows; the counts and tviol of the base are
+    // rebuilt by set_base and patched winner by winner, as topics_prepare / apply_winner_topics keep them
+    bool topics = false;
+    HostTopics ht;
+    std::vector<int4> tbnd;              // [T]
+    std::vector<uint16_t> tcnt, tlcnt;   // [T][32 W]
+    int tviol = 0;
+    TopicArgs ta{};
     std::string err;
 };
 
@@ -108,6 +118,33 @@ void rebuild_lists(Emu &e)
     }
 }
 
+// topics_prepare: the base's replicas and valid leaders per (topic, broker slot) (topic_count_kernel), then the
+// topic-row violation over every such cell (topic_violation_kernel)
+void count_topics(Emu &e)
+{
+    const HostModel &m = e.hm;
+    const int NSL = 32 * m.W;
+    e.tcnt.assign((size_t)e.ht.T * NSL, 0);
+    e.tlcnt.assign((size_t)e.ht.T * NSL, 0);
+    for (int p = 0; p < m.P; ++p) {
+        const size_t t = e.ht.topic_of[p];
+        const int ld = e.leader[p];
+        for (int s = 0; s < NSL; ++s) {
+            if (!((e.bits[(size_t)(s >> 5) * m.Ppad + p] >> (s & 31)) & 1u) || !broker_slot(&e.cs, m.B, s)) continue;
+            ++e.tcnt[t * NSL + s];
+            if (s == ld) ++e.tlcnt[t * NSL + s];
+        }
+    }
+    e.tviol = 0;
+    for (size_t i = 0; i < e.tcnt.size(); ++i) {
+        if (!broker_slot(&e.cs, m.B, (int)(i % NSL))) continue;
+        const int4 b = e.tbnd[i / NSL];
+        e.tviol += band_int(e.tcnt[i], b.x, b.y) + band_int(e.tlcnt[i], b.z, b.w);
+    }
+    e.ta.tcnt = e.tcnt.data();
+    e.ta.tlcnt = e.tlcnt.data();
+}
+
 void set_base(Emu &e, const std::vector<uint32_t> &bitsT, const std::vector<uint8_t> &leader)
 {
     const HostModel &m = e.hm;
@@ -123,6 +160,7 @@ void set_base(Emu &e, const std::vector<uint32_t> &bitsT, const std::vector<uint
     rebuild_lists(e);
     e.n_invalid = count_invalid(e);
     if (e.trans_ok) { if (m.W == 1) build_T<1>(e); else build_T<2>(e); }
+    if (e.topics) count_topics(e);
 }
 
 // State a search patches winner by winner, against the same state rebuilt from the current bits / leader: the one-hot
@@ -356,11 +394,12 @@ template <class F> auto dispatch(Emu &e, F f)
     return f(Run<EvalCfg<1, 5, 0, 0>>{});
 }
 
-// The HBM-base kernels of a replication session (kao_large.cu: search_large_kernel<W, false, true>,
-// eval_large_base_kernel<W, true>): their one evaluator configuration, every row's C1 / C7 operands from rftab.
+// The HBM-base kernels of a replication or topic session (kao_large.cu: search_large_kernel<W, kTopics, kRF>,
+// eval_large_base_kernel<W, kRF>): their one evaluator configuration; kRF: every row's C1 / C7 operands from rftab;
+// e.topics: the topic rows of kao_topics.cuh on top.
 template <int W> using LargeCfg = EvalCfg<W, 5, 0, kObjEntries>;
 
-template <int W> struct RunRf {
+template <int W, bool kRF> struct RunLarge {
     struct Totals {
         std::vector<int> cnt = std::vector<int>(256, 0), lcnt = std::vector<int>(256, 0), rc = std::vector<int>(32, 0);
         long long viol = 0, obj = 0;                   // raw, as block_eval leaves them in acc
@@ -377,7 +416,8 @@ template <int W> struct RunRf {
             for (int w = 0; w < W; ++w) x[w] = e.bits[(size_t)w * d.Ppad + p];
             const uint32_t ld = e.leader[p];
             int rv, ro;
-            row_eval<LargeCfg<W>, false, true>(d, m_obj, p, x, ld, rv, ro, row_rf(e.rftab.data(), p));
+            if constexpr (kRF) row_eval<LargeCfg<W>, false, true>(d, m_obj, p, x, ld, rv, ro, row_rf(e.rftab.data(), p));
+            else row_eval<LargeCfg<W>, false>(d, m_obj, p, x, ld, rv, ro);
             t.viol += rv;
             t.obj += ro;
             for (int w = 0; w < W; ++w)
@@ -392,6 +432,7 @@ template <int W> struct RunRf {
             t.viol += band_violation(t.cnt[s], e.cs.bnd_rep[s]) + band_violation(t.lcnt[s], e.cs.bnd_ldr[s]);
         for (int r = 0; r < d.R; ++r)
             t.viol += std::max(t.rc[r] - e.cs.rack_hi[r], 0) + std::max(e.cs.rack_lo[r] - t.rc[r], 0);
+        if (e.topics) t.viol += e.tviol;              // the search kernel adds tviol to block_eval's total
         return t;
     }
     // the per-thread generator on the base (its linear-scan form), as large_gen hands it to each thread
@@ -411,9 +452,14 @@ template <int W> struct RunRf {
         uint32_t rows[kMaxOps][W];
         gen(e, seed, round, idx, round_size, ps, rows);
         int viol, obj;
-        delta_eval<LargeCfg<W>, false, true>(e.prm, e.bits.data(), e.leader.data(), MemRef<false>(e.prm.swT), &e.cs, ps,
-                                             rows, t.cnt.data(), t.lcnt.data(), t.rc.data(), base_viol, base_obj, viol,
-                                             obj, e.rftab.data());
+        delta_eval<LargeCfg<W>, false, kRF>(e.prm, e.bits.data(), e.leader.data(), MemRef<false>(e.prm.swT), &e.cs, ps,
+                                            rows, t.cnt.data(), t.lcnt.data(), t.rc.data(), base_viol, base_obj, viol,
+                                            obj, kRF ? e.rftab.data() : nullptr);
+        if (e.topics) {
+            int rc[2 * kMaxOps], lc[2 * kMaxOps];
+            topic_events<W>(e.prm, e.ta, &e.cs, ps, rows, rc, lc);
+            viol += topic_delta<W>(e.ta, rc, lc);
+        }
         return pack_key(viol, obj, idx, e.prm.key_obj_bits);
     }
     // the base's (violation, objective) as the kernel hands it to delta_eval: the full pass, the violation clamped to int
@@ -453,6 +499,11 @@ template <int W> struct RunRf {
             PatchSet win;
             uint32_t rows[kMaxOps][W];
             gen(e, seed, round, (uint32_t)(best & kIdxMask), round_size, win, rows);
+            if (e.topics) {                           // apply_winner_topics: the winner's events against the base
+                int rc[2 * kMaxOps], lc[2 * kMaxOps];
+                topic_events<W>(e.prm, e.ta, &e.cs, win, rows, rc, lc);
+                topic_apply_events<W>(e.ta, rc, lc);
+            }
             for (int i = 0; i < win.n; ++i) {
                 for (int w = 0; w < W; ++w) e.bits[(size_t)w * e.hm.Ppad + win.p[i]] = rows[i][w];
                 e.leader[win.p[i]] = (uint8_t)win.ld[i];
@@ -462,15 +513,17 @@ template <int W> struct RunRf {
     }
 };
 
-template <class F> auto with_w(const Emu &e, F f)
+template <bool kRF, class F> auto with_w_rf(const Emu &e, F f)
 {
     switch (e.hm.W) {
-    case 1: return f(RunRf<1>{});
-    case 2: return f(RunRf<2>{});
-    case 4: return f(RunRf<4>{});
-    default: return f(RunRf<8>{});
+    case 1: return f(RunLarge<1, kRF>{});
+    case 2: return f(RunLarge<2, kRF>{});
+    case 4: return f(RunLarge<4, kRF>{});
+    default: return f(RunLarge<8, kRF>{});
     }
 }
+
+template <class F> auto with_w(const Emu &e, F f) { return e.rf ? with_w_rf<true>(e, f) : with_w_rf<false>(e, f); }
 
 // the device-side tables and Params of a session whose host model and evaluator configuration are set; its initial base
 void start(Emu &e)
@@ -548,6 +601,28 @@ void *kao_emu_create_replication(const kao_problem *pb, const kao_replication *r
     return e.release();
 }
 
+// kao_create_topics: a plain host model with topic rows, on the HBM-base path like a replication session; the rows as
+// build_host_topics checks them, the session's TopicArgs on the emulator's own tables
+void *kao_emu_create_topics(const kao_problem *pb, const kao_topics *tp)
+{
+    auto e = std::make_unique<Emu>();
+    if (!build_host_model(*pb, e->hm, g_err) || !build_host_topics(*pb, *tp, e->hm.Ppad, e->ht, g_err))
+        return nullptr;
+    e->hm.nplanes = 0;
+    e->hm.z_ok = false;
+    e->topics = true;
+    e->tbnd.resize(e->ht.T);
+    for (int t = 0; t < e->ht.T; ++t)
+        e->tbnd[t] = make_int4(e->ht.bnd[4 * t], e->ht.bnd[4 * t + 1], e->ht.bnd[4 * t + 2], e->ht.bnd[4 * t + 3]);
+    e->ta.T = e->ht.T;
+    e->ta.topic_of = e->ht.topic_of.data();
+    e->ta.bnd = e->tbnd.data();
+    e->ta.tviol = &e->tviol;
+    e->nph = 5; e->rack = 0; e->obj = kObjEntries;
+    start(*e);
+    return e.release();
+}
+
 int kao_emu_set_evaluator(void *h, int32_t mode)
 {
     Emu &e = *static_cast<Emu *>(h);
@@ -602,7 +677,7 @@ void kao_emu_get_base(void *h, int32_t *replicas, int64_t *violation, int64_t *o
     std::vector<uint32_t> bitsT(e.bits.begin(), e.bits.begin() + (size_t)e.hm.W * e.hm.Ppad);
     decode_replicas(e.hm, bitsT, e.leader, replicas);
     if (moves) *moves = count_moves(e.hm, replicas);
-    if (e.rf) {                                 // eval_large_base_kernel<W, true>: the raw violation
+    if (e.rf || e.topics) {                     // eval_large_base_kernel<W, kRF>: the raw violation (tviol added)
         with_w(e, [&](auto r) {
             const auto t = decltype(r)::base(e);
             if (violation) *violation = t.viol;
@@ -631,7 +706,7 @@ void kao_emu_candidate_keys(void *h, uint64_t seed, uint32_t round, uint32_t rou
 void kao_emu_search(void *h, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size, uint64_t *round_keys)
 {
     Emu &e = *static_cast<Emu *>(h);
-    if (e.rf) {
+    if (e.rf || e.topics) {
         with_w(e, [&](auto r) { decltype(r)::search(e, seed, first_round, rounds, round_size, round_keys); return 0; });
         return;
     }
@@ -651,7 +726,7 @@ int kao_emu_candidate_keys_delta(void *h, uint64_t seed, uint32_t round, uint32_
                                  uint32_t count, uint64_t *keys)
 {
     Emu &e = *static_cast<Emu *>(h);
-    if (e.rf) {
+    if (e.rf || e.topics) {
         with_w(e, [&](auto r) { decltype(r)::keys(e, seed, round, round_size, idx_begin, count, keys); return 0; });
         return 0;
     }

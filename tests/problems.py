@@ -308,3 +308,74 @@ def moved_base(pb, reps, seed):
     empty = (out < 0).all(1)
     out[empty] = reps[empty]                      # a short row that lost its last replica keeps it
     return out
+
+
+# ---- every one of the 256 slots a broker (docs/MODEL.md §2) -------------------------------------------------------
+# A cluster of 255 brokers grown by one: the current assignment uses brokers 0..254, the target list is 0..255 and
+# broker b sits in rack b // (256 / racks), so broker 255 is the last of the last rack, on slot 255, with no home
+# replica there (a home replica on slot 255 is DESIGN.md 7.1's known limit).  Slot 255 is then a real broker while
+# several tables use the byte 0xFF for "none" or "padding"; the new broker is empty, so every balance row that binds
+# on it (C3 / C4, and the topic rows of the labellings below) reads its slot.
+def grown_by_one(P, racks, RF=3, seed=0):
+    rng = np.random.RandomState(seed)
+    per = 256 // racks
+    current = [list(map(int, rng.choice(255, size=RF, replace=False))) for _ in range(P)]
+    return m.build_problem(current, list(range(256)), {b: "rack%02d" % (b // per) for b in range(256)}, RF)
+
+
+SLOT255_SHAPES = {
+    "s255_r32": lambda: grown_by_one(600, 32, seed=91),       # 32 racks of 8: 8-slot fields, KAO_MAX_RACKS
+    "s255_r16": lambda: grown_by_one(600, 16, seed=92),
+    "s255_r8": lambda: grown_by_one(500, 8, seed=93),         # 32-slot racks: one word each
+    "s255_r4": lambda: grown_by_one(500, 4, seed=94),         # 64-slot racks: two words each
+    "s255_r16_dense": lambda: with_dense_weights(grown_by_one(300, 16, seed=95), 95),
+    "s255_big": lambda: grown_by_one(9000, 16, seed=96),      # the HBM path without topic rows
+}
+
+
+def one_topic(pb):
+    """One topic over every partition: n RF >= 256 replicas, so its default rows bind on the empty broker 255"""
+    pb.topics = [("all", p) for p in range(pb.P)]
+    return pb
+
+
+def topics_of_sizes(pb, seed, top=600):
+    """Topics of 86..top partitions (seeded sizes, partitions interleaved by a seeded permutation), every one with
+    n RF >= 256 replicas: with the default rows each topic binds on broker 255"""
+    rng = np.random.RandomState(seed)
+    sizes = []
+    while sum(sizes) < pb.P:
+        sizes.append(min(int(rng.randint(-(-256 // pb.RF), top + 1)), pb.P - sum(sizes)))
+    if sizes[-1] * pb.RF < 256:                               # fold a short tail into the topic before it
+        tail = sizes.pop()
+        sizes[-1] += tail
+    label = np.repeat(np.arange(len(sizes)), sizes)[rng.permutation(pb.P)]
+    pb.topics = [("t%03d" % t, p) for p, t in enumerate(label)]
+    return pb
+
+
+# topic sessions with binding rows on broker 255, at and above 8,160 partitions
+SLOT255_TOPIC_SHAPES = {
+    "one_topic_r16": lambda: one_topic(SLOT255_SHAPES["s255_r16"]()),
+    "sized_r32": lambda: topics_of_sizes(grown_by_one(1200, 32, seed=97), 97),
+    "sized_r4": lambda: topics_of_sizes(SLOT255_SHAPES["s255_r4"](), 98, top=200),
+    "sized_big": lambda: topics_of_sizes(SLOT255_SHAPES["s255_big"](), 99),
+}
+
+
+def leader_on_255_rf_up():
+    """512 partitions on [p % 256, (p + 1) % 256], RF raised from 2 to 3, 256 brokers in 16 racks (broker b in rack
+    b % 16, so broker 255 is on slot 255): partitions 255 and 511 are led from slot 255 and their rows get completed"""
+    cur = [[p % 256, (p + 1) % 256] for p in range(512)]
+    return m.build_problem(cur, list(range(256)), {b: "r%02d" % (b % 16) for b in range(256)}, 3)
+
+
+def leader_on_255_removed():
+    """260 brokers, the last four removed, 16 racks of 16 among the 256 that stay: rows [p, p + 1, p + 2] mod 260,
+    so partitions 255 and 515 keep only their leader, on slot 255, and are completed"""
+    cur = [[p % 260, (p + 1) % 260, (p + 2) % 260] for p in range(520)]
+    return m.build_problem(cur, list(range(256)), {b: "r%02d" % (min(b, 255) // 16) for b in range(260)}, 3)
+
+
+# initial-base checks only: their current leaders sit on slot 255 (a home slot there, DESIGN.md 7.1), so no walks
+LEADER255_SHAPES = {"leader255_rf_up": leader_on_255_rf_up, "leader255_removed": leader_on_255_removed}

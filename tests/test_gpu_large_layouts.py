@@ -275,7 +275,7 @@ def test_one_topic_holding_65280_partitions(ref_lib):
 
 
 def test_one_topic_per_partition_at_65280_in_eight_word_rows(ref_lib):
-    """T = P = 65,280 at W = 8: 16.7 M (topic, slot) cells (DESIGN.md 7.2).  16 racks of up to 16, slot 255 padding."""
+    """T = P = 65,280 at W = 8: 16.7 M (topic, slot) cells (DESIGN.md 7.2).  16 racks of up to 16."""
     pb = make_problem(65280, [16] * 15 + [15], 3, seed=44, removed=3)
     pb.topics = [("t%d" % p, p) for p in range(pb.P)]
     tr = kao.topic_rows(kao.Problem.from_fields(pb))

@@ -208,23 +208,45 @@ def _sass(obj):
     return res
 
 
-def test_plain_and_topic_kernels_keep_their_pinned_sass():
-    """Every kernel of the large-path and engine objects as the build before the topic rows made it, and the topic search
-    kernels as the build before the per-partition rows made them: the plain search kernel became the kTopics = false
-    instantiation, with TopicArgs appended after every parameter it had, and then every search kernel became the
-    kRF = false instantiation, with the rftab pointer appended."""
+# the kTopics = true, kRF = false search kernels, as the pin file names them
+_TOPIC_SEARCH = re.compile(r"search_large_kernelILi\dELb1EEEv")
+
+
+def _check_pins(select):
+    """Every pinned kernel of tests/golden/sass_parent_large_engine.json whose pinned name `select` accepts against the
+    in-tree build -> how many were compared.  The plain search kernel became the kTopics = false instantiation, with
+    TopicArgs appended after every parameter it had, and then every search kernel became the kRF = false instantiation,
+    with the rftab pointer appended: the pinned names are mapped to the current ones."""
     _nvcc()
     pin = json.load(open(os.path.join(ROOT, "tests", "golden", "sass_parent_large_engine.json")))
+    n = 0
     for obj, kernels in pin["objects"].items():
         path = os.path.join(ROOT, "kafka_assignment_optimizer_b200", "_obj", obj)
         if not os.path.exists(path) or not shutil.which("cuobjdump"):
             pytest.skip("object files of the in-tree build or cuobjdump not available")
         now = _sass(path)
         for name, want in kernels.items():
+            if not select(name):
+                continue
             cur = re.sub(r"search_large_kernelILi(\d)EEEv(.*)$", r"search_large_kernelILi\1ELb0EEEv\g<2>9TopicArgs", name)
             cur = re.sub(r"search_large_kernelILi(\d)ELb(\d)EEEv(.*)$", r"search_large_kernelILi\1ELb\2ELb0EEEv\g<3>PKj", cur)
             ins = now[cur]
             assert (len(ins), hashlib.sha256("\n".join(ins).encode()).hexdigest()) == (want["instructions"], want["sha256"]), name
+            n += 1
+    return n
+
+
+def test_plain_and_replication_kernels_keep_their_pinned_sass():
+    """Every kernel of the large-path and engine objects other than the topic search kernels as the build before the
+    topic rows made it: neither the topic rows, the per-partition rows nor the topic functions in kao_topics.cuh
+    changed any of them."""
+    assert _check_pins(lambda name: not _TOPIC_SEARCH.search(name)) == 29
+
+
+def test_topic_search_kernels_keep_their_pinned_sass():
+    """The four topic search kernels (W = 1, 2, 4, 8) as the build that tells padding slots from broker slots by the
+    order index against B (kao_topics.cuh, broker_slot) made them: slot 255 is a broker when B = 256."""
+    assert _check_pins(lambda name: bool(_TOPIC_SEARCH.search(name))) == 4
 
 
 def test_submit_passes_topic_balance_only_when_asked():
