@@ -241,6 +241,38 @@ int kao_solve_replication(const kao_problem *pb, const kao_topics *tp, const kao
  * ppr_lo[p] .. ppr_hi[p].  replicas: a FEASIBLE assignment under those rows, [P*RF], leader first, -1 padded. */
 int kao_objective_bound_replication(const kao_problem *pb, const kao_replication *rp, const int32_t *replicas,
                                     int64_t *bound);
+
+/*
+ * Fixed partitions (docs/MODEL.md §12): "move these topics and leave everything else where it is".  fixed[p] = 1 keeps
+ * partition p exactly as cur[p] lists it (its non-negative entries in their order, the first one leading); its C1,
+ * C2/C5, C7 and per-partition replication rows leave the program, while its replicas still count in C3, C6 and C3t and
+ * its leader in C4 and C4t.  The call reduces the problem once on the host, to the searched rows with those loads moved
+ * into the bounds (band(c + f, lo, hi) = band(c, max(lo - f, 0), max(hi - f, 0)) + max(f - hi, 0)), and runs
+ * kao_solve_replication on it: the path, the options it accepts and its refusals (KAO_FLAG_ROW_MAJOR, sharding and
+ * KAO_FLAG_LP_BOUND above KAO_MAX_SMEM_PARTITIONS) follow from the REDUCED problem's size and rows.  A plain reduced
+ * problem of at most KAO_MAX_SMEM_PARTITIONS rows whose tables do not fit the shared memory of an SM (e.g. above 7,680
+ * rows at 33..64 broker slots) runs on the HBM path with uniform replication rows instead of being refused; there
+ * KAO_FLAG_ROW_MAJOR and sharding are KAO_E_ARG and KAO_FLAG_LP_BOUND is computed on the plain reduced problem.  Fixed topics drop
+ * out of the topic rows and the others are renumbered.
+ * Result: fixed rows come back as cur lists them (-1 padded to RF); violation = V' + V0 and objective = O' + O0, where
+ * V0 is what the fixed load alone exceeds (C3, C4, C6 and the cells of fixed topics) and O0 the fixed rows' objective;
+ * objective_bound = bound' + O0 (every bound); moves counts the searched rows; feasible = (violation == 0), so the call
+ * returns KAO_INFEASIBLE when V0 > 0 whatever the search found; optimal keeps its meaning.  key and key_obj_bits are
+ * those of the reduced search.
+ * KAO_E_ARG before any CUDA call, besides what kao_solve_replication refuses: a fixed row that is empty, that names a
+ * broker after a -1 (a replica outside the target list cannot be kept), that names one broker twice or more than RF;
+ * with topic rows a topic that is partly fixed; every partition fixed.  fixed == NULL: exactly kao_solve_replication.
+ * The session API (kao_create*) and kao_eval take no mask: their callers build the problem they search.
+ */
+int kao_solve_fixed(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, const uint8_t *fixed,
+                    const kao_options *opt, kao_result *res);
+/* kao_objective_bound_replication of the reduced problem of kao_solve_fixed, plus O0: an upper bound on the objective
+ * of every feasible assignment that keeps the fixed rows.  Host-side, needs no GPU.  replicas == NULL: the cheap bound;
+ * else a [P*RF] assignment whose searched rows are feasible in the reduced problem (its fixed rows are not read): the
+ * flow bound.  fixed == NULL: exactly kao_objective_bound_replication. */
+int kao_objective_bound_fixed(const kao_problem *pb, const kao_replication *rp, const uint8_t *fixed,
+                              const int32_t *replicas, int64_t *bound);
+
 int kao_destroy(kao_handle *h);
 /* base <- current assignment restricted to the target brokers and completed to RF (MODEL §4) */
 int kao_reset(kao_handle *h);

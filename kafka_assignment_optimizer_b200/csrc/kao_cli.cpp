@@ -119,6 +119,9 @@ struct Model {
     std::vector<int32_t> topic_of, trep_lo, trep_hi, tldr_lo, tldr_hi;
     // per-partition C1 / C7 rows (docs/MODEL.md §11, --keep-rf / --topic-rf): empty when every partition has RF
     std::vector<int32_t> prf, pprlo, pprhi;
+    // fixed rows (docs/MODEL.md §12, --topics-to-move): empty when every row is searched
+    std::vector<uint8_t> fixed;
+    bool is_fixed(int p) const { return !fixed.empty() && fixed[p]; }
 };
 
 static int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
@@ -219,58 +222,129 @@ Model build_model_rf(const std::vector<Row> &rows, const std::vector<int> &broke
     return m;
 }
 
-// lp_solve LP-format text, same families and naming as README.md:144-185
+// --topics-to-move (docs/MODEL.md §12): Kafka's topics-to-move.json names the topics to reassign; a row is searched when
+// its topic is listed or when it has a replica on a broker outside the target list (that data has to move), every
+// other row is fixed.  A fixed row must be one kao_solve_fixed keeps: non-empty, distinct brokers, at most RF of them
+// (checked here, so that --emit-lp refuses what the solve refuses).  With topic rows (topic_balance) no topic may be
+// partly fixed, which the removal of a broker causes when a topic with a replica there is not listed.
+void fix_rows(Model &m, const std::set<std::string> &move, const std::vector<int> &brokers,
+              const std::map<std::string, int> &topic_rf, bool topic_balance)
+{
+    for (const std::string &t : move)
+        if (std::find(m.topic_names.begin(), m.topic_names.end(), t) == m.topic_names.end())
+            throw std::runtime_error("--topics-to-move: no topic named " + t + " in the assignment");
+    const std::set<int> ids(brokers.begin(), brokers.end());
+    m.fixed.assign(m.P, 0);
+    for (int p = 0; p < m.P; ++p) {
+        bool leaves = false;
+        for (int b : m.rows[p].replicas) leaves |= !ids.count(b);
+        m.fixed[p] = !move.count(m.rows[p].topic) && !leaves;
+        if (!m.fixed[p]) continue;
+        const Row &r = m.rows[p];
+        const std::string at = "--topics-to-move: partition " + r.topic + "-" + std::to_string(r.partition);
+        if (topic_rf.count(r.topic))
+            throw std::runtime_error("--topic-rf: topic " + r.topic + " has fixed partitions (not in --topics-to-move)");
+        if (r.replicas.empty()) throw std::runtime_error(at + " is kept but has no replica");
+        if ((int)std::set<int>(r.replicas.begin(), r.replicas.end()).size() != (int)r.replicas.size())
+            throw std::runtime_error(at + " is kept but lists a broker twice");
+        if ((int)r.replicas.size() > m.RF)
+            throw std::runtime_error(at + " is kept but has more than RF = " + std::to_string(m.RF) + " replicas");
+    }
+    if (!topic_balance) return;
+    for (size_t t = 0; t < m.topic_names.size(); ++t) {
+        int nfix = 0, n = 0;
+        for (int p = 0; p < m.P; ++p)
+            if (m.topic_of[p] == (int)t) { ++n; nfix += m.fixed[p]; }
+        if (nfix && nfix < n)
+            throw std::runtime_error("--topics-to-move with --topic-balance: topic " + m.topic_names[t] + " is partly fixed (" +
+                                     std::to_string(n - nfix) + " of its " + std::to_string(n) + " partitions have a replica "
+                                     "on a broker outside --brokers); with topic rows a topic is moved or kept whole: "
+                                     "add it to the topics to move");
+    }
+}
+
+// lp_solve LP-format text, same families and naming as README.md:144-185.  With fixed rows: the restricted program,
+// the variables of the searched rows only and the right-hand sides of C3 / C4 / C6 / topic rows less the fixed load
+// (not clamped: a negative one is a row the fixed load alone exceeds), the fixed rows' objective O0 in a comment
 void emit_lp(const Model &m, std::ostream &o, bool topics)
 {
     auto var = [&](int b, int p, bool l) {
         return "t1b" + std::to_string(m.broker_ids[b]) + "p" + std::to_string(p) + (l ? "_l" : "");
     };
+    // the fixed load: replicas and leaders per broker, replicas per rack, per (topic, broker); the fixed objective
+    const size_t T = m.topic_names.size();
+    std::vector<long> f(m.B, 0), fl(m.B, 0), fr(m.R, 0), ft(T * m.B, 0), flt(T * m.B, 0);
+    long O0 = 0;
+    int nfixed = 0;
+    for (int p = 0; p < m.P; ++p) {
+        if (!m.is_fixed(p)) continue;
+        ++nfixed;
+        bool led = false;
+        for (int i = 0; i < m.RFcur; ++i) {
+            const int b = m.cur[(size_t)p * m.RFcur + i];
+            if (b < 0) continue;
+            ++f[b]; ++fr[m.rack_of[b]]; ++ft[(size_t)m.topic_of[p] * m.B + b];
+            if (!led) { ++fl[b]; ++flt[(size_t)m.topic_of[p] * m.B + b]; O0 += m.wL[(size_t)p * m.B + b]; led = true; }
+            else O0 += m.wF[(size_t)p * m.B + b];
+        }
+    }
+    if (!m.fixed.empty())
+        o << "// Fixed partitions: " << nfixed << ", objective of the fixed partitions O0 = " << O0 << "\n";
     o << "// Optimization function, based on current assignment\nmax: ";
     bool first = true;
     for (int p = 0; p < m.P; ++p)
-        for (int b = 0; b < m.B; ++b) {
+        for (int b = 0; b < m.B && !m.is_fixed(p); ++b) {
             const int f = m.wF[(size_t)p * m.B + b], l = m.wL[(size_t)p * m.B + b];
             if (f) { o << (first ? "" : " + ") << f << " " << var(b, p, false); first = false; }
             if (l) { o << (first ? "" : " + ") << l << " " << var(b, p, true); first = false; }
         }
     o << ";\n\n// Constrain on replication factor for every partition\n";
     for (int p = 0; p < m.P; ++p) {
+        if (m.is_fixed(p)) continue;
         for (int b = 0; b < m.B; ++b) o << (b ? " + " : "") << var(b, p, false) << " + " << var(b, p, true);
         o << " = " << (m.prf.empty() ? m.RF : m.prf[p]) << ";\n";
     }
     o << "\n// Constraint on having one and only one leader per partition\n";
     for (int p = 0; p < m.P; ++p) {
+        if (m.is_fixed(p)) continue;
         for (int b = 0; b < m.B; ++b) o << (b ? " + " : "") << var(b, p, true);
         o << " = 1;\n";
     }
     o << "\n// Constraint on min/max replicas per broker\n";
     for (int b = 0; b < m.B; ++b)
         for (int pass = 0; pass < 2; ++pass) {
-            for (int p = 0; p < m.P; ++p) o << (p ? " + " : "") << var(b, p, false) << " + " << var(b, p, true);
-            o << (pass ? " >= " : " <= ") << (pass ? m.rep_lo[b] : m.rep_hi[b]) << ";\n";
+            bool f2 = true;
+            for (int p = 0; p < m.P; ++p)
+                if (!m.is_fixed(p)) { o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true); f2 = false; }
+            o << (pass ? " >= " : " <= ") << (pass ? m.rep_lo[b] : m.rep_hi[b]) - f[b] << ";\n";
         }
     o << "\n// Constraint on min/max leaders per broker\n";
     for (int b = 0; b < m.B; ++b)
         for (int pass = 0; pass < 2; ++pass) {
-            for (int p = 0; p < m.P; ++p) o << (p ? " + " : "") << var(b, p, true);
-            o << (pass ? " >= " : " <= ") << (pass ? m.ldr_lo[b] : m.ldr_hi[b]) << ";\n";
+            bool f2 = true;
+            for (int p = 0; p < m.P; ++p)
+                if (!m.is_fixed(p)) { o << (f2 ? "" : " + ") << var(b, p, true); f2 = false; }
+            o << (pass ? " >= " : " <= ") << (pass ? m.ldr_lo[b] : m.ldr_hi[b]) - fl[b] << ";\n";
         }
     o << "\n// Constraint on no leader and replicas on the same broker\n";
     for (int b = 0; b < m.B; ++b)
-        for (int p = 0; p < m.P; ++p) o << var(b, p, false) << " + " << var(b, p, true) << " <= 1;\n";
+        for (int p = 0; p < m.P; ++p)
+            if (!m.is_fixed(p)) o << var(b, p, false) << " + " << var(b, p, true) << " <= 1;\n";
     for (int r = 0; r < m.R; ++r) {
         o << "\n// Constrain on min/max total replicas per racks. " << m.rack_names[r] << " here\n";
         for (int pass = 0; pass < 2; ++pass) {
             bool f2 = true;
             for (int b = 0; b < m.B; ++b) {
                 if (m.rack_of[b] != r) continue;
-                for (int p = 0; p < m.P; ++p) { o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true); f2 = false; }
+                for (int p = 0; p < m.P; ++p)
+                    if (!m.is_fixed(p)) { o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true); f2 = false; }
             }
-            o << (pass ? " >= " : " <= ") << (pass ? m.rack_lo[r] : m.rack_hi[r]) << ";\n";
+            o << (pass ? " >= " : " <= ") << (pass ? m.rack_lo[r] : m.rack_hi[r]) - fr[r] << ";\n";
         }
     }
     o << "\n// Constrain on min/max replicas per partitions per racks.\n";
     for (int p = 0; p < m.P; ++p) {
+        if (m.is_fixed(p)) continue;
         const int plo = m.prf.empty() ? m.ppr_lo : m.pprlo[p], phi = m.prf.empty() ? m.ppr_hi : m.pprhi[p];
         for (int r = 0; r < m.R; ++r)
             for (int pass = 0; pass < (plo > 0 ? 2 : 1); ++pass) {
@@ -284,25 +358,32 @@ void emit_lp(const Model &m, std::ostream &o, bool topics)
     }
     for (int t = 0; topics && t < (int)m.topic_names.size(); ++t)
         for (int kind = 0; kind < 2; ++kind) {
+            bool searched = false;                      // a wholly fixed topic's rows have no variables: left out
+            for (int p = 0; p < m.P; ++p) searched |= m.topic_of[p] == t && !m.is_fixed(p);
+            if (!searched) continue;
             o << "\n// Constraint on min/max " << (kind ? "leaders" : "replicas") << " of topic " << m.topic_names[t]
               << " per broker\n";
             for (int b = 0; b < m.B; ++b)
                 for (int pass = 0; pass < 2; ++pass) {
                     bool f2 = true;
                     for (int p = 0; p < m.P; ++p) {
-                        if (m.topic_of[p] != t) continue;
+                        if (m.topic_of[p] != t || m.is_fixed(p)) continue;
                         if (!kind) o << (f2 ? "" : " + ") << var(b, p, false) << " + " << var(b, p, true);
                         else o << (f2 ? "" : " + ") << var(b, p, true);
                         f2 = false;
                     }
+                    const long shift = (kind ? flt : ft)[(size_t)t * m.B + b];
                     const int lo = kind ? m.tldr_lo[t] : m.trep_lo[t], hi = kind ? m.tldr_hi[t] : m.trep_hi[t];
-                    o << (pass ? " >= " : " <= ") << (pass ? lo : hi) << ";\n";
+                    o << (pass ? " >= " : " <= ") << (pass ? lo : hi) - shift << ";\n";
                 }
         }
     o << "\n// All variables are binary\nbin\n";
+    first = true;
     for (int p = 0; p < m.P; ++p)
-        for (int b = 0; b < m.B; ++b)
-            o << (p || b ? ", " : "") << var(b, p, false) << ", " << var(b, p, true);
+        for (int b = 0; b < m.B && !m.is_fixed(p); ++b) {
+            o << (first ? "" : ", ") << var(b, p, false) << ", " << var(b, p, true);
+            first = false;
+        }
     o << ";\n";
 }
 
@@ -329,7 +410,7 @@ int usage()
     std::fprintf(stderr,
                  "usage: kao-cli --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
                  "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--topic-balance] [--emit-lp] [--stats]\n"
-                 "               [--keep-rf] [--topic-rf name:N,...]\n");
+                 "               [--keep-rf] [--topic-rf name:N,...] [--topics-to-move FILE]\n");
     return 2;
 }
 
@@ -389,6 +470,14 @@ int main(int argc, char **argv)
         Model m = keep_rf || !topic_rf.empty()
                       ? build_model_rf(rows, brokers, racks, keep_rf, a.count("rf") ? rf : 0, topic_rf)
                       : build_model(rows, brokers, racks, rf);
+        if (a.count("topics-to-move")) {                      // Kafka's {"topics":[{"topic":...}],"version":1}
+            const std::string move_text = slurp(a["topics-to-move"]);
+            Parser pt(move_text);
+            const Json tdoc = pt.value();
+            std::set<std::string> move;
+            for (const Json &e : tdoc.at("topics").arr) move.insert(e.at("topic").str);
+            fix_rows(m, move, brokers, topic_rf, topic_balance && !emit);   // --emit-lp shifts each (topic, broker) row
+        }
         if (emit) { emit_lp(m, std::cout, topic_balance); return 0; }
 
         kao_problem pb{};
@@ -416,14 +505,19 @@ int main(int argc, char **argv)
         kao_topics tp{(int32_t)m.topic_names.size(), m.topic_of.data(), m.trep_lo.data(), m.trep_hi.data(),
                       m.tldr_lo.data(), m.tldr_hi.data()};
         kao_replication rp{m.prf.data(), m.pprlo.data(), m.pprhi.data()};
-        const int rc = !m.prf.empty() ? kao_solve_replication(&pb, topic_balance ? &tp : nullptr, &rp, &opt, &res)
+        const int rc = !m.fixed.empty() ? kao_solve_fixed(&pb, topic_balance ? &tp : nullptr, m.prf.empty() ? nullptr : &rp,
+                                                          m.fixed.data(), &opt, &res)
+                       : !m.prf.empty() ? kao_solve_replication(&pb, topic_balance ? &tp : nullptr, &rp, &opt, &res)
                        : topic_balance ? kao_solve_topics(&pb, &tp, &opt, &res) : kao_solve(&pb, &opt, &res);
         if (rc < 0) { std::fprintf(stderr, "kao-cli: %s\n", kao_last_error()); return 1; }
         if (rc == KAO_INFEASIBLE)
             std::fprintf(stderr, "kao-cli: warning: no assignment satisfying every constraint was found (violation %lld)\n",
                          (long long)res.violation);
         std::cout << "{\"version\":1,\"partitions\":[\n";
+        int last = m.P - 1;                                   // only the searched rows, as Kafka's --generate
+        while (last > 0 && m.is_fixed(last)) --last;
         for (int p = 0; p < m.P; ++p) {
+            if (m.is_fixed(p)) continue;
             std::cout << "    {\"topic\":\"" << m.rows[p].topic << "\",\"partition\":" << m.rows[p].partition << ",\"replicas\":[";
             bool first = true;
             for (int i = 0; i < m.RF; ++i) {
@@ -432,15 +526,17 @@ int main(int argc, char **argv)
                 std::cout << (first ? "" : ",") << m.broker_ids[b];
                 first = false;
             }
-            std::cout << "]}" << (p + 1 < m.P ? "," : "") << "\n";
+            std::cout << "]}" << (p < last ? "," : "") << "\n";
         }
         std::cout << "]}\n";
         if (stats)
             std::fprintf(stderr, "kao-cli: objective %lld (upper bound %lld%s), violation %lld, replica moves %d, %llu candidates, "
-                                 "%d GPU(s), %.2f ms on device, %.2f ms total\n",
+                                 "%d GPU(s), %.2f ms on device, %.2f ms total%s\n",
                          (long long)res.objective, (long long)res.objective_bound, res.optimal ? ": proven optimal" : "",
                          (long long)res.violation, res.moves, (unsigned long long)res.n_candidates, res.n_gpus, res.device_ms,
-                         res.total_ms);
+                         res.total_ms,
+                         m.fixed.empty() ? "" : (", " + std::to_string(std::count(m.fixed.begin(), m.fixed.end(), 1)) +
+                                                 " partitions fixed").c_str());
         return rc == KAO_INFEASIBLE ? 3 : 0;
     } catch (const std::exception &e) {
         std::fprintf(stderr, "kao-cli: %s\n", e.what());

@@ -426,6 +426,18 @@ static int reset_impl(kao_handle *h)
     return upload_base(h, bitsT, leader);
 }
 
+// the shared-memory plan of a session below kSmemRowsMax partitions: mask planes + one-hot plane next to the base when
+// they fit, else packed entries / the dense table (m.nplanes = 0); false when even that exceeds an SM's 227 KB
+static bool fit_smem_plan(HostModel &m, int threads, SmemPlan &plan)
+{
+    plan = make_plan(m.W, m.Ppad, threads / 32, m.nplanes > 0 ? m.nplanes * m.W : 4, m.P, m.RF, m.nplanes > 0);
+    if (plan.total > 227u * 1024u && m.nplanes > 0) {
+        m.nplanes = 0;
+        plan = make_plan(m.W, m.Ppad, threads / 32, 4, m.P, m.RF, false);
+    }
+    return plan.total <= 227u * 1024u;
+}
+
 static int create_impl(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, int32_t device,
                        kao_handle *h)
 {
@@ -457,13 +469,7 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, const kao_re
         h->hm.z_ok = false;
     } else {
         h->threads = W <= 2 ? KAO_THREADS : KAO_THREADS_WIDE;
-        h->plan = make_plan(W, Ppad, h->threads / 32, m.nplanes > 0 ? m.nplanes * W : 4, m.P, m.RF, m.nplanes > 0);
-        if (h->plan.total > 227u * 1024u && m.nplanes > 0) {
-            // mask planes + one-hot plane do not fit next to the base: score with packed entries / the dense table
-            h->hm.nplanes = 0;
-            h->plan = make_plan(W, Ppad, h->threads / 32, 4, m.P, m.RF, false);
-        }
-        if (h->plan.total > 227u * 1024u)
+        if (!fit_smem_plan(h->hm, h->threads, h->plan))
             return fail(KAO_E_ARG, "problem too large for the shared-memory resident search kernel");
         // column-major evaluator: 8-slot rack fields, C7 = "at most one replica per rack", an objective that fits
         // eight term planes (kao_host.hpp); its two transposed planes (2 * W words per partition) and the term planes
@@ -1267,6 +1273,106 @@ static int solve_impl(const kao_problem *pb, const kao_topics *tp, const kao_rep
     return KAO_OK;
 }
 
+// fixed partitions (docs/MODEL.md §12): solve the reduced problem, then put the fixed rows and constants back.  A reduced
+// problem of at most kSmemRowsMax plain rows whose tables do not fit the shared memory of an SM (at 33..64 slots above
+// 7,680 rows) would be refused by the shared-memory path, although the cluster it came from runs on the HBM path: it
+// runs there too, with uniform replication rows (rf[p] = RF, ppr = pb's C7: the same program), and keeps the LP
+// certificate, computed here on the plain reduced problem.
+static int solve_fixed_impl(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, const uint8_t *fixed,
+                            const kao_options *opt, kao_result *res)
+{
+    if (!fixed) return solve_impl(pb, tp, rp, opt, res);
+    if (!pb || !opt || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
+    const auto t0 = std::chrono::steady_clock::now();
+    FixedReduction fr;
+    std::string why;
+    if (!reduce_fixed(*pb, tp, rp, fixed, fr, why)) return fail(KAO_E_ARG, why);
+    kao_options o = *opt;
+    const kao_replication *rrp = rp ? &fr.rp : nullptr;
+    std::vector<int32_t> urf, ulo, uhi;
+    kao_replication uniform{};
+    bool lp_here = false;
+    if (!tp && !rp && fr.pb.P <= kSmemRowsMax) {
+        HostModel m;
+        SmemPlan plan;
+        if (!build_host_model(fr.pb, m, why)) return fail(KAO_E_ARG, why);
+        if (!fit_smem_plan(m, m.W <= 2 ? KAO_THREADS : KAO_THREADS_WIDE, plan)) {
+            const std::string on = "the reduced problem (" + std::to_string(fr.pb.P) +
+                                   " rows) does not fit the shared memory of an SM and runs on the HBM path, which offers no ";
+            if (o.flags & KAO_FLAG_ROW_MAJOR) return fail(KAO_E_ARG, "KAO_FLAG_ROW_MAJOR: " + on + "evaluator choice");
+            if ((o.n_gpus > 1 || __builtin_popcount(o.device_mask) > 1) && !(o.flags & KAO_FLAG_SPREAD_RESTARTS))
+                return fail(KAO_E_ARG, "n_gpus > 1 without KAO_FLAG_SPREAD_RESTARTS: " + on + "sharded rounds");
+            urf.assign(fr.pb.P, pb->RF); ulo.assign(fr.pb.P, pb->ppr_lo); uhi.assign(fr.pb.P, pb->ppr_hi);
+            uniform = kao_replication{urf.data(), ulo.data(), uhi.data()};
+            rrp = &uniform;
+            lp_here = (o.flags & KAO_FLAG_LP_BOUND) != 0;
+            if (lp_here && !lp_bound_fits(fr.pb)) return fail(KAO_E_ARG, std::string("KAO_FLAG_LP_BOUND: ") + kLpLimit);
+            o.flags &= ~KAO_FLAG_LP_BOUND;
+        }
+    }
+    // solve_impl writes into a copy, so that the caller's result never points at the local buffer
+    std::vector<int32_t> reduced((size_t)fr.pb.P * pb->RF, -1);
+    kao_result r = *res;
+    r.replicas = reduced.data();
+    const int rc = solve_impl(&fr.pb, tp ? &fr.tp : nullptr, rrp, &o, &r);
+    if (rc != KAO_OK && rc != KAO_INFEASIBLE) return rc;
+    if (lp_here && r.feasible) {
+        std::vector<int> devs;
+        int64_t lp = 0;
+        uint32_t its = 0;
+        int lrc = pick_devices(opt, devs);
+        if (lrc != KAO_OK) return lrc;
+        lrc = lagrange_bound_device(fr.pb, devs[0], r.objective, KAO_LP_ITERATIONS, wait_budget_ns(), &lp, &its, nullptr,
+                                    nullptr, why);
+        if (lrc != KAO_OK) return fail(lrc, why);
+        r.objective_bound = std::min(r.objective_bound, lp);
+        r.optimal = r.feasible && r.objective == r.objective_bound;
+    }
+    int32_t *const out = res->replicas;
+    *res = r;
+    res->replicas = out;
+    expand_fixed(*pb, fr, reduced.data(), out);
+    res->violation += fr.V0;
+    res->objective += fr.O0;
+    res->objective_bound += fr.O0;
+    res->feasible = res->violation == 0;
+    res->optimal = res->feasible && res->objective == res->objective_bound;
+    res->total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (!res->feasible) {
+        g_err = fr.V0 ? "the fixed partitions alone violate C3, C4, C6 or a fixed topic's rows" : "no candidate satisfying C1..C7 was found";
+        return KAO_INFEASIBLE;
+    }
+    return KAO_OK;
+}
+
+static int objective_bound_fixed_impl(const kao_problem *pb, const kao_replication *rp, const uint8_t *fixed,
+                                      const int32_t *replicas, int64_t *bound)
+{
+    if (!pb || !bound) return fail(KAO_E_ARG, "null argument");
+    FixedReduction fr;
+    std::string why;
+    const kao_problem *q = pb;
+    const kao_replication *qr = rp;
+    std::vector<int32_t> sub;
+    if (fixed) {
+        if (!reduce_fixed(*pb, nullptr, rp, fixed, fr, why)) return fail(KAO_E_ARG, why);
+        q = &fr.pb;
+        qr = rp ? &fr.rp : nullptr;
+        if (replicas) {
+            sub.resize((size_t)fr.pb.P * pb->RF);
+            for (size_t k = 0; k < fr.searched.size(); ++k)
+                std::memcpy(&sub[k * pb->RF], replicas + (size_t)fr.searched[k] * pb->RF, (size_t)pb->RF * 4);
+            replicas = sub.data();
+        }
+    }
+    HostModel m;
+    if (!build_host_model(*q, m, why) || (qr && !build_host_replication(*qr, m, why))) return fail(KAO_E_ARG, why);
+    *bound = objective_upper_bound(m, *q);
+    if (replicas) *bound = objective_flow_bound(m, *q, replicas, *bound);
+    *bound += fr.O0;
+    return KAO_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // the C ABI (include/kao.h): thin, guarded entry points
 // ------------------------------------------------------------------------------------------
@@ -1484,4 +1590,14 @@ extern "C" int kao_solve_replication(const kao_problem *pb, const kao_topics *tp
                                      const kao_options *opt, kao_result *res)
 {
     return guarded([&] { return solve_impl(pb, tp, rp, opt, res); });
+}
+extern "C" int kao_solve_fixed(const kao_problem *pb, const kao_topics *tp, const kao_replication *rp, const uint8_t *fixed,
+                               const kao_options *opt, kao_result *res)
+{
+    return guarded([&] { return solve_fixed_impl(pb, tp, rp, fixed, opt, res); });
+}
+extern "C" int kao_objective_bound_fixed(const kao_problem *pb, const kao_replication *rp, const uint8_t *fixed,
+                                         const int32_t *replicas, int64_t *bound)
+{
+    return guarded([&] { return objective_bound_fixed_impl(pb, rp, fixed, replicas, bound); });
 }

@@ -481,6 +481,145 @@ inline std::vector<uint32_t> replication_table(const HostModel &m)
     return t;
 }
 
+// Fixed partitions (docs/MODEL.md §12): the problem over the searched rows only.  A fixed row keeps cur[p] exactly, so
+// its C1, C2/C5 and C7 rows leave the program and its load on brokers, racks and topics becomes a constant.  Since
+//   band(c + f, lo, hi) = band(c, max(lo - f, 0), max(hi - f, 0)) + max(f - hi, 0)    for every c >= 0, lo <= hi,
+// that constant moves into the bounds of C3 / C4 / C6 and into V0; the fixed rows' objective terms sum to O0.  Fully
+// fixed topics drop out (their C3t / C4t cells are constants of V0), the others are renumbered in ascending order.  The
+// kao_problem / kao_topics / kao_replication below point into this struct's own tables.
+struct FixedReduction {
+    std::vector<int32_t> searched;            // [P'] original index of each searched row, ascending
+    std::vector<uint16_t> wF, wL;
+    std::vector<int32_t> cur, rep_lo, rep_hi, ldr_lo, ldr_hi, rack_lo, rack_hi;
+    std::vector<int32_t> rf, ppr_lo, ppr_hi;                          // with replication rows
+    std::vector<int32_t> topic_of, trep_lo, trep_hi, tldr_lo, tldr_hi;  // with topic rows
+    kao_problem pb{};
+    kao_topics tp{};
+    kao_replication rp{};
+    int64_t V0 = 0, O0 = 0;
+};
+
+inline int64_t band(int64_t c, int64_t lo, int64_t hi) { return std::max<int64_t>(lo - c, 0) + std::max<int64_t>(c - hi, 0); }
+
+// Validates pb (and tp / rp) as kao_solve_replication does, then the fixed rows: each one non-empty, its brokers dense
+// indices before any -1, distinct, at most RF of them; with topic rows no topic partly fixed; at least one row searched.
+inline bool reduce_fixed(const kao_problem &pb, const kao_topics *tp, const kao_replication *rp, const uint8_t *fixed,
+                         FixedReduction &fr, std::string &why)
+{
+    auto bad = [&](const std::string &s) { why = "fixed partitions: " + s; return false; };
+    HostModel m;
+    HostTopics ht;
+    if (!build_host_model(pb, m, why) || (rp && !build_host_replication(*rp, m, why)) ||
+        (tp && !build_host_topics(pb, *tp, m.Ppad, ht, why, rp ? rp->rf : nullptr)))
+        return false;
+    if (!fixed) return bad("null mask");
+    const int P = pb.P, B = pb.B, R = pb.R, RFc = pb.RFcur;
+    std::vector<int64_t> f(B, 0), fl(B, 0), fr_r(R, 0);
+    fr.searched.clear();
+    fr.V0 = fr.O0 = 0;
+    for (int p = 0; p < P; ++p) {
+        if (!fixed[p]) { fr.searched.push_back(p); continue; }
+        const int32_t *row = pb.cur + (size_t)p * RFc;
+        const std::string at = "row " + std::to_string(p);
+        int n = 0;
+        for (int i = 0; i < RFc; ++i) {
+            if (row[i] < 0) continue;
+            if (row[i] >= B) return bad(at + " names broker " + std::to_string(row[i]) + ", not a dense index 0..B-1");
+            if (n < i) return bad(at + " has a broker after a -1: a replica outside the target list cannot be kept");
+            for (int k = 0; k < i; ++k)
+                if (row[k] == row[i]) return bad(at + " lists broker " + std::to_string(row[i]) + " twice");
+            ++n;
+        }
+        if (n == 0) return bad(at + " is empty");
+        if (n > pb.RF) return bad(at + " has more than RF = " + std::to_string(pb.RF) + " replicas");
+        for (int i = 0; i < n; ++i) {
+            const int b = row[i];
+            ++f[b];
+            ++fr_r[pb.rack_of[b]];
+            fr.O0 += i == 0 ? pb.wL[(size_t)p * B + b] : pb.wF[(size_t)p * B + b];
+        }
+        ++fl[row[0]];
+    }
+    const int Pn = (int)fr.searched.size();
+    if (Pn == 0) return bad("every partition is fixed");
+    // topics: a topic is searched when one of its partitions is, and then must be searched whole
+    std::vector<int32_t> new_topic;
+    if (tp) {
+        std::vector<int> nfix(tp->T, 0), nsearch(tp->T, 0);
+        for (int p = 0; p < P; ++p) ++(fixed[p] ? nfix : nsearch)[tp->topic_of[p]];
+        new_topic.assign(tp->T, -1);
+        fr.trep_lo.clear(); fr.trep_hi.clear(); fr.tldr_lo.clear(); fr.tldr_hi.clear();
+        for (int t = 0; t < tp->T; ++t) {
+            if (nfix[t] && nsearch[t])
+                return bad("topic " + std::to_string(t) + " of kao_topics is partly fixed (" + std::to_string(nfix[t]) + " of " +
+                           std::to_string(nfix[t] + nsearch[t]) + " partitions): with topic rows a topic is fixed or "
+                           "searched whole, so move it whole or keep all of it");
+            if (!nsearch[t]) continue;
+            new_topic[t] = (int32_t)fr.trep_lo.size();
+            fr.trep_lo.push_back(tp->rep_lo[t]); fr.trep_hi.push_back(tp->rep_hi[t]);
+            fr.tldr_lo.push_back(tp->ldr_lo[t]); fr.tldr_hi.push_back(tp->ldr_hi[t]);
+        }
+        // the C3t / C4t cells of every fixed topic, over all B brokers
+        std::vector<int64_t> cnt((size_t)tp->T * B, 0), lcnt((size_t)tp->T * B, 0);
+        for (int p = 0; p < P; ++p) {
+            if (!fixed[p]) continue;
+            const int t = tp->topic_of[p];
+            const int32_t *row = pb.cur + (size_t)p * RFc;
+            for (int i = 0; i < RFc && row[i] >= 0; ++i) ++cnt[(size_t)t * B + row[i]];
+            ++lcnt[(size_t)t * B + row[0]];
+        }
+        for (int t = 0; t < tp->T; ++t)
+            if (new_topic[t] < 0)
+                for (int b = 0; b < B; ++b)
+                    fr.V0 += band(cnt[(size_t)t * B + b], tp->rep_lo[t], tp->rep_hi[t]) +
+                             band(lcnt[(size_t)t * B + b], tp->ldr_lo[t], tp->ldr_hi[t]);
+    }
+    // the bounds, shifted by the fixed load
+    auto shift = [&](const int32_t *lo, const int32_t *hi, const std::vector<int64_t> &load, int n,
+                     std::vector<int32_t> &nlo, std::vector<int32_t> &nhi) {
+        nlo.resize(n); nhi.resize(n);
+        for (int i = 0; i < n; ++i) {
+            nlo[i] = (int32_t)std::max<int64_t>(lo[i] - load[i], 0);
+            nhi[i] = (int32_t)std::max<int64_t>(hi[i] - load[i], 0);
+            fr.V0 += std::max<int64_t>(load[i] - hi[i], 0);
+        }
+    };
+    shift(pb.rep_lo, pb.rep_hi, f, B, fr.rep_lo, fr.rep_hi);
+    shift(pb.ldr_lo, pb.ldr_hi, fl, B, fr.ldr_lo, fr.ldr_hi);
+    shift(pb.rack_lo, pb.rack_hi, fr_r, R, fr.rack_lo, fr.rack_hi);
+    // the searched rows, in order
+    fr.wF.resize((size_t)Pn * B); fr.wL.resize((size_t)Pn * B); fr.cur.resize((size_t)Pn * RFc);
+    fr.rf.clear(); fr.ppr_lo.clear(); fr.ppr_hi.clear(); fr.topic_of.clear();
+    for (int k = 0; k < Pn; ++k) {
+        const int p = fr.searched[k];
+        std::memcpy(&fr.wF[(size_t)k * B], pb.wF + (size_t)p * B, (size_t)B * 2);
+        std::memcpy(&fr.wL[(size_t)k * B], pb.wL + (size_t)p * B, (size_t)B * 2);
+        std::memcpy(&fr.cur[(size_t)k * RFc], pb.cur + (size_t)p * RFc, (size_t)RFc * 4);
+        if (rp) { fr.rf.push_back(rp->rf[p]); fr.ppr_lo.push_back(rp->ppr_lo[p]); fr.ppr_hi.push_back(rp->ppr_hi[p]); }
+        if (tp) fr.topic_of.push_back(new_topic[tp->topic_of[p]]);
+    }
+    fr.pb = pb;
+    fr.pb.P = Pn;
+    fr.pb.wF = fr.wF.data(); fr.pb.wL = fr.wL.data(); fr.pb.cur = fr.cur.data();
+    fr.pb.rep_lo = fr.rep_lo.data(); fr.pb.rep_hi = fr.rep_hi.data();
+    fr.pb.ldr_lo = fr.ldr_lo.data(); fr.pb.ldr_hi = fr.ldr_hi.data();
+    fr.pb.rack_lo = fr.rack_lo.data(); fr.pb.rack_hi = fr.rack_hi.data();
+    fr.tp = kao_topics{(int32_t)fr.trep_lo.size(), fr.topic_of.data(), fr.trep_lo.data(), fr.trep_hi.data(),
+                       fr.tldr_lo.data(), fr.tldr_hi.data()};
+    fr.rp = kao_replication{fr.rf.data(), fr.ppr_lo.data(), fr.ppr_hi.data()};
+    return true;
+}
+
+// [P'*RF] replica lists of the reduced problem -> [P*RF] of pb: searched rows as found, fixed rows as cur lists them
+inline void expand_fixed(const kao_problem &pb, const FixedReduction &fr, const int32_t *reduced, int32_t *replicas)
+{
+    for (int p = 0; p < pb.P; ++p)
+        for (int i = 0; i < pb.RF; ++i)
+            replicas[(size_t)p * pb.RF + i] = i < pb.RFcur ? std::max<int32_t>(pb.cur[(size_t)p * pb.RFcur + i], -1) : -1;
+    for (size_t k = 0; k < fr.searched.size(); ++k)
+        std::memcpy(replicas + (size_t)fr.searched[k] * pb.RF, reduced + k * pb.RF, (size_t)pb.RF * 4);
+}
+
 inline void fill_consts(const HostModel &m, Consts &cs)
 {
     for (int s = 0; s < 256; ++s) {

@@ -11,7 +11,7 @@ from typing import Optional
 import numpy as np
 
 from .problem import (Problem, ReplicationRows, TopicRows, build_problem, parse_assignment_json, parse_broker_list, parse_rack_map,
-                      reassignment_json, topic_rows)
+                      parse_topics_to_move, reassignment_json, topic_rows)
 
 _LIB_PATH = os.environ.get("KAO_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libkao.so")
 KAO_OK, KAO_INFEASIBLE = 0, 1
@@ -95,7 +95,11 @@ def objective_bound(pb: Problem, replicas=None) -> int:
     out = C.c_int64()
     r = None if replicas is None else np.ascontiguousarray(replicas, dtype=np.int32)
     rp = None if r is None else C.c_void_p(r.ctypes.data)
-    if pb.replication is None:
+    if pb.fixed is not None:    # fixed rows (docs/MODEL.md §12): the bound of the reduced problem plus their objective
+        cr, fx = _CReplication(pb.replication), _fixed(pb)
+        _check(load_library().kao_objective_bound_fixed(_CProblem(pb).ref(), cr.ref(), C.c_void_p(fx.ctypes.data), rp,
+                                                        C.byref(out)))
+    elif pb.replication is None:
         _check(load_library().kao_objective_bound(_CProblem(pb).ref(), rp, C.byref(out)))
     else:       # per-partition rows: kao_objective_bound_replication (rf[p] replicas per row)
         cr = _CReplication(pb.replication)
@@ -111,6 +115,7 @@ def lp_bound(pb: Problem, replicas, device: int = 0, max_iterations: int = LP_IT
     """The Lagrangian LP bound of kao_lp_bound (docs/MODEL.md 9; GPU): an upper bound on the objective of every
     feasible assignment, aimed at the objective of `replicas` (a feasible assignment [P, RF], leader first).  -> (bound,
     iterations run), or (bound, iterations run, multipliers int64[2B + R] with LP_FRACTION_BITS fractional bits)."""
+    _refuse_fixed(pb, "lp_bound")
     if pb.replication is not None:
         raise ValueError("lp_bound: the Lagrangian LP bound is built for one RF and one C7 row for every partition "
                          "(docs/MODEL.md 9), not for per-partition replication factors")
@@ -123,6 +128,19 @@ def lp_bound(pb: Problem, replicas, device: int = 0, max_iterations: int = LP_IT
                                        C.c_uint32(max_iterations), C.byref(out), C.byref(its),
                                        C.c_void_p(u.ctypes.data)))
     return (out.value, its.value, u) if multipliers else (out.value, its.value)
+
+
+def _fixed(pb: Problem) -> np.ndarray:
+    fx = np.ascontiguousarray(pb.fixed, dtype=np.uint8)
+    if fx.shape != (pb.P,):
+        raise ValueError("fixed must be [P]")
+    return fx
+
+
+def _refuse_fixed(pb: Problem, what: str):
+    if pb.fixed is not None:
+        raise ValueError("%s: a problem with fixed rows is searched through solve (kao_solve_fixed); the session API and "
+                         "kao_eval take the problem they search, e.g. the reduced one (docs/MODEL.md §12)" % what)
 
 
 class _CProblem:
@@ -167,14 +185,16 @@ class _KaoReplication(C.Structure):
 
 
 class _CReplication:
-    """kao_replication over contiguous copies of a ReplicationRows."""
+    """kao_replication over contiguous copies of a ReplicationRows (None: no replication rows, a NULL pointer)."""
 
-    def __init__(self, rr: ReplicationRows):
-        self.keep = [np.ascontiguousarray(x, dtype=np.int32) for x in (rr.rf, rr.ppr_lo, rr.ppr_hi)]
-        self.c = _KaoReplication(*(x.ctypes.data for x in self.keep))
+    def __init__(self, rr: Optional[ReplicationRows]):
+        self.c = None
+        if rr is not None:
+            self.keep = [np.ascontiguousarray(x, dtype=np.int32) for x in (rr.rf, rr.ppr_lo, rr.ppr_hi)]
+            self.c = _KaoReplication(*(x.ctypes.data for x in self.keep))
 
     def ref(self):
-        return C.byref(self.c)
+        return None if self.c is None else C.byref(self.c)
 
 
 @dataclasses.dataclass
@@ -202,6 +222,7 @@ class Session:
     without topics, and also searches with delta evaluation only."""
 
     def __init__(self, pb: Problem, device: int = 0, topics: Optional[TopicRows] = None):
+        _refuse_fixed(pb, "Session")
         self.pb = pb
         self._cp = _CProblem(pb)
         self._h = C.c_void_p()
@@ -376,7 +397,9 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
     bound (KAO_FLAG_BOUND) / also from the Lagrangian LP bound (KAO_FLAG_LP_BOUND); either can prove optimality.
     topic_balance: every topic spread over the brokers too (kao_solve_topics with `topics`, by default
     topic_rows(pb)); the bounds then leave the topic rows out and may be looser.  A problem with per-partition rows
-    (pb.replication) is solved through kao_solve_replication."""
+    (pb.replication) is solved through kao_solve_replication, one with fixed rows (pb.fixed, build_problem(topics_to_move=
+    ...)) through kao_solve_fixed: only the other rows are searched, the fixed ones come back as pb.cur lists them, and
+    topic_balance then needs every topic fixed or searched whole (docs/MODEL.md §12)."""
     lib = load_library()
     cp = _CProblem(pb)
     if topic_balance and topics is None:
@@ -387,7 +410,18 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
     opt = _KaoOptions(seed & (2 ** 64 - 1), rounds, round_size, device, flags, n_gpus, device_mask)
     res = _KaoResult()
     res.replicas = reps.ctypes.data
-    if pb.replication is not None:
+    if pb.fixed is not None:
+        if topics is not None:          # a topic is moved or kept whole (docs/MODEL.md §12): name the ones that are not
+            t_of, fx = np.asarray(topics.topic_of), np.asarray(pb.fixed, bool)
+            part = [t for t in range(topics.T) if fx[t_of == t].any() and not fx[t_of == t].all()]
+            if part:
+                raise ValueError("topic rows with fixed partitions: a topic is moved or kept whole, and these topics are "
+                                 "partly fixed (a partition on a leaving broker is searched): %s; add them to the topics "
+                                 "to move" % ", ".join(str(topics.names[t]) if topics.names else str(t) for t in part))
+        ct, cr, fx = _CTopics(topics), _CReplication(pb.replication), _fixed(pb)
+        rc = _check(lib.kao_solve_fixed(cp.ref(), ct.ref(), cr.ref(), C.c_void_p(fx.ctypes.data), C.byref(opt), C.byref(res)),
+                    allow_infeasible=not require_feasible)
+    elif pb.replication is not None:
         ct, cr = _CTopics(topics), _CReplication(pb.replication)
         rc = _check(lib.kao_solve_replication(cp.ref(), ct.ref(), cr.ref(), C.byref(opt), C.byref(res)),
                     allow_infeasible=not require_feasible)
@@ -406,6 +440,7 @@ def evaluate(pb: Problem, replicas, device: int = 0):
     """GPU evaluation of explicit assignments: replicas [n, P, RF] (or [P, RF]) -> (violation[n],
     objective[n]).  Not for a problem with per-partition rows (pb.replication): kao_eval scores C1 / C7 against RF;
     Session(pb).get_base() evaluates such a problem's base."""
+    _refuse_fixed(pb, "evaluate")
     if pb.replication is not None:
         raise ValueError("evaluate: kao_eval scores C1 / C7 against one RF; a problem with per-partition replication "
                          "factors is evaluated through a Session (set_base, get_base)")
@@ -433,14 +468,18 @@ class AssignmentOptimizer:
         self.solve_options = solve_options
 
     def optimize(self, assignment_json, broker_list, rack_map, rf: Optional[int] = None, keep_rf: bool = False,
-                 topic_rf: Optional[dict] = None):
+                 topic_rf: Optional[dict] = None, topics_to_move=None):
         """keep_rf: every topic keeps the length of its longest replica list; topic_rf {name: RF}: those topics take
-        that RF, the others keep theirs (keep_rf) or take `rf` (build_problem)."""
+        that RF, the others keep theirs (keep_rf) or take `rf` (build_problem).  topics_to_move: a list of topic names
+        or Kafka's topics-to-move.json document ({"topics": [{"topic": name}], "version": 1}); only those topics and the
+        partitions that must leave a broker are searched, and only they are in the returned reassignment."""
         rows, topics = parse_assignment_json(assignment_json)
         brokers = parse_broker_list(broker_list) if isinstance(broker_list, str) else list(broker_list)
         racks = parse_rack_map(rack_map) if isinstance(rack_map, str) else dict(rack_map)
         if rf is None and not (keep_rf or topic_rf):
             rf = max(len(r) for r in rows)
-        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf)
+        if topics_to_move is not None:
+            topics_to_move = parse_topics_to_move(topics_to_move)
+        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf, topics_to_move=topics_to_move)
         res = solve(pb, self.seed, self.rounds, self.round_size, self.device, **self.solve_options)
         return reassignment_json(pb, res.replicas), res

@@ -39,6 +39,7 @@ class Problem:
     broker_ids: np.ndarray  # int32  [B]      dense index -> Kafka broker id
     topics: Optional[list] = None   # per-row (topic, partition)
     replication: Optional["ReplicationRows"] = None   # per-partition C1 / C7 rows (docs/MODEL.md §11), None: RF for all
+    fixed: Optional[np.ndarray] = None  # bool [P]: rows kept exactly as cur lists them (docs/MODEL.md §12), None: none
 
     @classmethod
     def from_fields(cls, other) -> "Problem":
@@ -101,13 +102,39 @@ def partition_rf(current: Sequence[Sequence[int]], topics: Optional[list], rf: O
     return out
 
 
+def fixed_rows(current: Sequence[Sequence[int]], broker_ids: Iterable[int], topics: Optional[list],
+               topics_to_move: Iterable[str]) -> np.ndarray:
+    """The rows a reassignment of `topics_to_move` (Kafka's topics-to-move.json) keeps as they are (docs/MODEL.md §12):
+    every row except those of the listed topics and those with a replica on a broker outside `broker_ids`, whose data
+    has to move.  Rows without topics form the one topic "t1"; a listed name the rows do not contain is a ValueError."""
+    names = [t[0] if topics else "t1" for t in (topics or [None] * len(current))]
+    move = {str(t) for t in topics_to_move}
+    unknown = sorted(move - set(names))
+    if unknown:
+        raise ValueError("topics_to_move names topics the assignment does not contain: %s" % ", ".join(unknown))
+    ids = {int(b) for b in broker_ids}
+    return np.array([n not in move and all(int(b) in ids for b in reps) for n, reps in zip(names, current)], bool)
+
+
 def build_problem(current: Sequence[Sequence[int]], broker_ids: Iterable[int],
                   rack_by_broker: Dict[int, str], rf: Optional[int], topics: Optional[list] = None,
-                  keep_rf: bool = False, topic_rf: Optional[Dict[str, int]] = None) -> Problem:
+                  keep_rf: bool = False, topic_rf: Optional[Dict[str, int]] = None,
+                  topics_to_move: Optional[Iterable[str]] = None) -> Problem:
     """keep_rf / topic_rf (partition_rf): every topic keeps its own replication factor, or takes the one named for it.
     When the partitions then differ, RF becomes the largest of them (the width of every replica list), C3 / C6 follow
     from the sum of the per-partition factors and the problem carries per-partition rows (ReplicationRows, C7 = floor /
-    ceil of rf[p] / R); when they all agree the problem is the plain one with that RF."""
+    ceil of rf[p] / R); when they all agree the problem is the plain one with that RF.  topics_to_move: only those
+    topics (and the rows that must leave a broker) are searched, every other row is fixed (Problem.fixed, fixed_rows);
+    topic_rf may then name only searched topics."""
+    if topics_to_move is not None:
+        fixed = fixed_rows(current, broker_ids, topics, topics_to_move)
+        names = [t[0] if topics else "t1" for t in (topics or [None] * len(current))]
+        pinned = sorted({n for n, f in zip(names, fixed) if f} & set(topic_rf or {}))
+        if pinned:
+            raise ValueError("topic_rf names topics whose partitions are fixed: %s" % ", ".join(pinned))
+        pb = build_problem(current, broker_ids, rack_by_broker, rf, topics, keep_rf, topic_rf)
+        pb.fixed = fixed
+        return pb
     if keep_rf or topic_rf:
         rfs = partition_rf(current, topics, rf, keep_rf, topic_rf)
         pb = build_problem(current, broker_ids, rack_by_broker, int(rfs.max()), topics)
@@ -195,6 +222,15 @@ def parse_assignment_json(text: str):
     return [list(map(int, e["replicas"])) for e in parts], [(e["topic"], int(e["partition"])) for e in parts]
 
 
+def parse_topics_to_move(doc) -> List[str]:
+    """Kafka's `topics-to-move.json` ({"topics": [{"topic": name}, ...], "version": 1}, README.md:35-48), as text or
+    parsed; a plain list of names is taken as it is."""
+    doc = json.loads(doc) if isinstance(doc, str) else doc
+    if isinstance(doc, dict):
+        return [str(e["topic"]) for e in doc["topics"]]
+    return [str(t) for t in doc]
+
+
 def parse_broker_list(text: str) -> List[int]:
     """`--broker-list 0,1,...,18` (README.md:48)."""
     return [int(t) for t in str(text).replace(" ", "").split(",") if t != ""]
@@ -213,9 +249,12 @@ def parse_rack_map(text: str) -> Dict[int, str]:
 
 def reassignment_json(pb: Problem, replicas: np.ndarray) -> dict:
     """`--reassignment-json-file` document (README.md:67-78, :88): same shape as the input,
-    leader (preferred replica) first."""
+    leader (preferred replica) first.  With fixed rows (pb.fixed) only the searched partitions, as Kafka's
+    `--generate` lists only the topics to move."""
     parts = []
     for p in range(pb.P):
+        if pb.fixed is not None and pb.fixed[p]:
+            continue
         topic, part = pb.topics[p] if pb.topics else ("t1", p)
         parts.append({"topic": topic, "partition": part,
                       "replicas": [int(pb.broker_ids[b]) for b in replicas[p] if b >= 0]})

@@ -8,7 +8,8 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
                    "racks": "0:a,1:b,...",                               README.md:27-29
                    "rf": 2, "rounds": 256, "round_size": 32768, "restarts": 1, "patience": 0, "delta": false,
                    "gpus": 1, "spread_restarts": false, "certificate": false,
-                   "lp_certificate": false, "topic_balance": false, "keep_rf": false, "topic_rf": {}}
+                   "lp_certificate": false, "topic_balance": false, "keep_rf": false, "topic_rf": {},
+                   "topics_to_move": ["name", ...]}
     200           {"reassignment": {"version":1,"partitions":[...]},    README.md:67-78
                    "objective": ..., "violation": ..., "moves": ..., "feasible": ...,
                    "objective_bound": ..., "proven_optimal": ...}
@@ -20,6 +21,9 @@ optima the flow bound cannot, e.g. after brokers are removed.  `topic_balance` a
 brokers (the per-topic rows of docs/MODEL.md §10, default bounds of `topic_rows`).  `keep_rf` keeps every topic's own
 replication factor (the length of its longest replica list) and `topic_rf` ({"topic": N}) sets it for the named
 topics, the others keeping theirs or taking `rf` when it is given (per-partition rows, docs/MODEL.md §11).
+`topics_to_move` searches only those topics and the partitions that must leave a broker, keeps every other partition
+where it is (still counted in every balance row, docs/MODEL.md §12) and returns only the searched partitions, as
+`kafka-reassign-partitions --generate` does for its topics-to-move.json.
 
 `python -m kafka_assignment_optimizer_b200.service --port 8080` (needs a GPU: there is no CPU path).
 """
@@ -30,7 +34,8 @@ import json
 from http.server import BaseHTTPRequestHandler, ThreadingHTTPServer
 from typing import Callable, Optional
 
-from .problem import build_problem, parse_assignment_json, parse_broker_list, parse_rack_map, reassignment_json
+from .problem import (build_problem, parse_assignment_json, parse_broker_list, parse_rack_map, parse_topics_to_move,
+                      reassignment_json)
 
 
 MAX_ROUNDS = 1 << 20            # KAO_MAX_ROUNDS
@@ -53,14 +58,16 @@ def handle_submit(body: dict, solver: Optional[Callable] = None) -> dict:
     racks = body["racks"]
     racks = parse_rack_map(racks) if isinstance(racks, str) else {int(k): str(v) for k, v in racks.items()}
     keep_rf, topic_rf = bool(body.get("keep_rf", False)), body.get("topic_rf") or None
+    # fixed rows (docs/MODEL.md §12), only when the request lists topics to move
+    move = {"topics_to_move": parse_topics_to_move(body["topics_to_move"])} if "topics_to_move" in body else {}
     if keep_rf or topic_rf:
         # per-partition replication factors (docs/MODEL.md §11): the problem carries them to the solver
         rf = int(body["rf"]) if body.get("rf") else None
         topic_rf = {str(k): int(v) for k, v in topic_rf.items()} if topic_rf else None
-        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf)
+        pb = build_problem(rows, brokers, racks, rf, topics, keep_rf=keep_rf, topic_rf=topic_rf, **move)
     else:
         rf = int(body.get("rf") or max(len(r) for r in rows))
-        pb = build_problem(rows, brokers, racks, rf, topics)
+        pb = build_problem(rows, brokers, racks, rf, topics, **move)
     if solver is None:
         from .optimizer import solve as solver
     # a request cannot ask for an unbounded search: the limits of include/kao.h, checked here as well
