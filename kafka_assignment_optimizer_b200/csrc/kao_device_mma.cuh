@@ -30,7 +30,7 @@ constexpr int kSPlanes = 4;          // max(0, RF - n) < 16 (RF < 16: rf_mask ho
 // PTX: ldmatrix of four 8 x 16-byte matrices and the binary MMA.  A fragment (m16 x k256, row):
 // a0 = row g, 32-bit word t of the k-step; a1 = row g + 8, word t; a2 / a3 = the same rows, word t + 4.
 // B fragment (k256 x n8, col): b0 = column g, word t; b1 = column g, word t + 4.  D: d0 / d1 = row g, columns 2 t,
-// 2 t + 1; d2 / d3 = row g + 8.  (g = lane / 4, t = lane % 4.)  tests/emu_mma/mma_emu.hpp restates both.
+// 2 t + 1; d2 / d3 = row g + 8.  (g = lane / 4, t = lane % 4.)  tests/emu/mma_emu.hpp restates both.
 // ------------------------------------------------------------------------------------------
 #if !defined(KAO_HOST_EMU)
 __device__ __forceinline__ void ldsm_x4(const uint32_t *row, uint32_t (&a)[4])

@@ -7,7 +7,8 @@
 // cross-GPU exchange) are only tested on the GPU.  Replication sessions (kao_emu_create_replication) run the kRF forms
 // of the row and delta evaluators on the HBM-base kernels' configuration (tests/test_replication_emulation.py); topic
 // sessions (kao_emu_create_topics) add the topic rows of csrc/kao_topics.cuh to it (tests/test_slot255_cpu.py).
-// Never linked into libkao.so.
+// tensor_core.cpp (the tensor-core body) and reduce_fixed.cpp (the fixed-partition reduction) are included at the end:
+// one translation unit, one library, tests/emu/_build/libkao_emu.so.  Never linked into libkao.so.
 #define KAO_HOST_EMU 1
 #include "warp_emu.hpp"
 
@@ -806,3 +807,6 @@ void kao_emu_eval(void *h, const int32_t *replicas, int32_t n, int64_t *violatio
 }
 
 }  // extern "C"
+
+#include "tensor_core.cpp"
+#include "reduce_fixed.cpp"

@@ -2,34 +2,21 @@
 LP bound (docs/MODEL.md §9) that the CUDA kernel is compared with bit for bit.  Never part of the product."""
 import ctypes as C
 import os
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, "lagrange_ref.c")
 _lib = None
 
 
-def _build():
-    out_dir = os.path.join(_HERE, "_build")
-    try:
-        os.makedirs(out_dir, exist_ok=True)
-        if not os.access(out_dir, os.W_OK):
-            raise OSError
-    except OSError:
-        out_dir = tempfile.mkdtemp(prefix="kao_lp_ref_")
-    so = os.path.join(out_dir, "liblagrange_ref.so")
-    if not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(_SRC):
-        subprocess.check_call(["gcc", "-O2", "-std=c11", "-Wall", "-Wextra", "-fPIC", "-shared", "-o", so, _SRC])
-    return so
-
-
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(_build())
+        _lib = C.CDLL(native.shared_library(os.path.join(_HERE, "_build"), "liblagrange_ref.so",
+                                            ["gcc", "-O2", "-std=c11", "-Wall", "-Wextra", "-fPIC", "-shared", _SRC], [_SRC]))
         _lib.lagrange_ref_box.restype = C.c_int64
     return _lib
 

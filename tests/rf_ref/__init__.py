@@ -4,11 +4,10 @@ oracle/kao_ref.c and tests/topics_ref) and the rows put into oracle.model's eval
 of the product."""
 import ctypes as C
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
 import topics_ref
 from oracle import model, ref
 
@@ -19,24 +18,11 @@ _DEPS = (_SRC, os.path.join(_ROOT, "oracle", "kao_ref.c"), os.path.join(_ROOT, "
 _lib = None
 
 
-def _build():
-    out_dir = os.path.join(_HERE, "_build")
-    try:
-        os.makedirs(out_dir, exist_ok=True)
-        if not os.access(out_dir, os.W_OK):
-            raise OSError
-    except OSError:
-        out_dir = tempfile.mkdtemp(prefix="kao_rf_ref_")
-    so = os.path.join(out_dir, "libkao_rf_ref.so")
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(d) for d in _DEPS):
-        subprocess.check_call(["gcc", "-O3", "-fopenmp", "-fPIC", "-std=c11", "-shared", "-o", so, _SRC])
-    return so
-
-
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(_build())
+        _lib = C.CDLL(native.shared_library(os.path.join(_HERE, "_build"), "libkao_rf_ref.so",
+                                            ["gcc", "-O3", "-fopenmp", "-fPIC", "-std=c11", "-shared", _SRC], _DEPS))
         _lib.kao_rref_search.restype = C.c_uint64
     return _lib
 

@@ -1,5 +1,5 @@
 """Fixed partitions (docs/MODEL.md §12) without a GPU: the engine's host reduction (reduce_fixed, compiled for the host
-by tests/emu_fixed) scored by the emulated sessions of tests/emu, plus V0 / O0, is the restricted program of
+by tests/emu) scored by the emulated sessions of the same library, plus V0 / O0, is the restricted program of
 tests/fixed_ref.py; kao_objective_bound_fixed brackets the HiGHS restricted optimum; every refusal is KAO_E_ARG before
 any CUDA call; `kao-cli --emit-lp --topics-to-move` writes the restricted program; the Python codec and /submit pick
 the searched rows by the CLI's rule."""
@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 from scipy.optimize import Bounds, LinearConstraint, milp
 
-import emu_fixed
+import emu
 import fixed_ref as F
 import kafka_assignment_optimizer_b200 as kao
 from emu import EmuSession
@@ -32,7 +32,7 @@ PLAIN = ["readme", "readme_tb", "cfg2", "cfg2_rm2", "cfg3_small", "w4_s16", "w8_
 
 
 def _full(pb, red, reduced):
-    out = emu_fixed.expand(pb, np.isin(np.arange(pb.P), red.searched, invert=True), reduced)
+    out = emu.expand(pb, np.isin(np.arange(pb.P), red.searched, invert=True), reduced)
     assert np.array_equal(out, F.expand(pb, red, reduced))
     return out
 
@@ -41,7 +41,7 @@ def _check(opb, fx, tr=None, rr=None, seeds=(0, 1)):
     """reduce_fixed against the restatement, then the emulated reduced session + V0 / O0 against the restricted program
     at the reduced problem's initial base and at moved bases"""
     pb = kao.Problem.from_fields(opb)
-    red = emu_fixed.reduce(pb, fx, tr, rr)
+    red = emu.reduce(pb, fx, tr, rr)
     want = F.reduce(pb, fx, tr, rr)
     assert (red.V0, red.O0) == (want.V0, want.O0) and np.array_equal(red.searched, want.searched)
     for k in ("cur", "wF", "wL", "rep_lo", "rep_hi", "ldr_lo", "ldr_hi", "rack_lo", "rack_hi"):
@@ -198,7 +198,7 @@ def test_refusals_without_a_gpu():
     fx[np.flatnonzero(fx)[0]] = False
     rc, _, msg = _solve_rc(tp, fx, tr)
     assert rc == -1 and "partly fixed" in msg
-    emu_fixed.reduce(tp, fx)
+    emu.reduce(tp, fx)
     # what kao_solve_replication refuses is still refused first
     rc, rcb, msg = _solve_rc(dataclasses.replace(pb, ppr_lo=64, ppr_hi=64), one)
     assert rc == -1 and rcb == -1 and "per-partition-per-rack" in msg

@@ -1,5 +1,5 @@
 """The column-major evaluator with its sums on the tensor cores (csrc/kao_device_mma.cuh, schedules with pop 0x100)
-under the warp emulator (tests/emu_mma on top of tests/emu): ldmatrix and the binary MMA are restated with their PTX
+under the warp emulator (tests/emu, pop 0x100): ldmatrix and the binary MMA are restated with their PTX
 fragment layouts, and 32 candidates are generated, parked and evaluated together as one warp of the search kernel does it.
 Keys and trajectories must be the restatement's, bit for bit."""
 import numpy as np
@@ -27,11 +27,8 @@ def emu():
 
 
 @pytest.fixture(scope="module")
-def mma():
-    import emu_mma
-
-    emu_mma.lib()
-    return emu_mma
+def mma(emu):
+    return lambda pb: emu.MmaSession(pb, 0x100)
 
 
 def product(pb):
@@ -41,7 +38,7 @@ def product(pb):
 def check(mma, ref_lib, pb, rounds=3, size=256, n=96):
     r = ref_lib.Ref(pb)
     bits, ld = r.init_base()
-    sess = mma.MmaSession(product(pb))
+    sess = mma(product(pb))
     for rnd in (2, 3):                                                    # round 3: a cycle round
         want = r.candidate_keys(bits, ld, 0xC0FFEE, rnd, 1024, 1024 - n, n)
         assert (want == sess.candidate_keys(0xC0FFEE, rnd, 1024, 1024 - n, n)).all(), rnd
@@ -68,7 +65,7 @@ def test_mma_body_on_the_layout_shapes_it_covers(emu, mma, ref_lib):
             check(mma, ref_lib, pb, rounds=3, size=128, n=64)
         else:
             with pytest.raises(ValueError):
-                mma.MmaSession(product(pb))
+                mma(product(pb))
     assert {"planes8_w1", "planes8_w2"} <= set(covered)
 
 
@@ -84,7 +81,7 @@ def test_mma_body_on_short_rows_and_invalid_leaders(emu, mma, ref_lib, name):
     form of the column-major evaluator, and the base evaluates like the exact model."""
     pb = SHAPES_MMA[name]()
     r = ref_lib.Ref(pb)
-    sess = mma.MmaSession(product(pb))
+    sess = mma(product(pb))
     pop = emu.EmuSession(product(pb))
     assert pop.set_evaluator(1)
     rng = np.random.RandomState(5)

@@ -1,5 +1,5 @@
 """The sorted-batch body of the tensor-core schedules (pop 0x300, csrc/kao_kernels.cuh: build_cand_list and the batch loop)
-restated under the warp emulator (tests/emu_sorted, on top of tests/emu_mma): every CTA sorts its share of a round by the class of the candidates'
+restated under the warp emulator (tests/emu): every CTA sorts its share of a round by the class of the candidates'
 control words (csrc/kao_device_mma.cuh, cand_class) and generates batches of 32 neighbours of that order.  Keys must be
 the oracle restatement's, bit for bit, whichever lanes share a batch."""
 import numpy as np
@@ -13,10 +13,10 @@ SEED = 0xC0FFEE
 
 @pytest.fixture(scope="module")
 def srt():
-    import emu_sorted
+    import emu
 
-    emu_sorted.lib()
-    return emu_sorted
+    emu.lib()
+    return emu
 
 
 @pytest.fixture(scope="module")
@@ -24,7 +24,7 @@ def cfg3(srt, ref_lib):
     pb = m.synthetic_problem(1000, 64, 8, 3)
     r = ref_lib.Ref(pb)
     bits, ld = r.init_base()
-    sess = srt.SortedSession(kao.Problem.from_fields(pb))
+    sess = srt.MmaSession(kao.Problem.from_fields(pb), 0x300)
     yield sess, r, bits, ld
     sess.close()
 

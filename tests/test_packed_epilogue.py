@@ -1,5 +1,5 @@
 """The packed MMA epilogue (csrc/kao_device_mma.cuh, the sorted-batch schedule pop 0x300: two candidates per 16 x 2
-instruction) under the warp emulator (tests/emu_packed on top of tests/emu_mma).  Keys and trajectories must be the
+instruction) under the warp emulator (tests/emu, pop 0x300).  Keys and trajectories must be the
 restatement's, bit for bit, including bounds far above the column totals (clamped to P), bounds of 0, and the largest
 column-major row count.  The host forms of the intrinsics are held to a plain-integer model first."""
 import dataclasses
@@ -53,16 +53,16 @@ def with_random_bounds(pb, seed):
 
 @pytest.fixture(scope="module")
 def packed():
-    import emu_packed
+    import emu
 
-    emu_packed.lib()
-    return emu_packed
+    emu.lib()
+    return emu
 
 
 def check(packed, ref_lib, pb, rounds=3, size=256, n=96):
     r = ref_lib.Ref(pb)
     bits, ld = r.init_base()
-    sess = packed.PackedSession(kao.Problem.from_fields(pb))
+    sess = packed.MmaSession(kao.Problem.from_fields(pb), 0x300)
     for rnd in (2, 3):                                                    # round 3: a cycle round
         want = r.candidate_keys(bits, ld, 0xC0FFEE, rnd, 1024, 1024 - n, n)
         assert (want == sess.candidate_keys(0xC0FFEE, rnd, 1024, 1024 - n, n)).all(), rnd

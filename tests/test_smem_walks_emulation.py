@@ -1,5 +1,5 @@
 """Walks of the shared-memory search kernel's column-major forms under the warp emulators (tests/emu: popcount forms
-1-6, tests/emu_mma: the tensor-core body), with the state every winner patches checked against the same state rebuilt
+1-6 and the tensor-core body), with the state every winner patches checked against the same state rebuilt
 from the base every 10 rounds (kao_emu_check_state): the transposed, term, rack-field and shortfall planes t_patch_row
 rewrites, the leader one-hot plane, the count of invalid leaders that decides whether the leader plane answers the
 generator, and the displaced lists.  A mis-patched plane that never changes a winner is invisible to every GPU
@@ -41,11 +41,8 @@ def emu():
 
 
 @pytest.fixture(scope="module")
-def mma():
-    import emu_mma
-
-    emu_mma.lib()
-    return emu_mma
+def mma(emu):
+    return lambda pb: emu.MmaSession(pb, 0x100)
 
 
 def product(pb):
@@ -79,7 +76,7 @@ def test_patched_state_equals_the_rebuilt_state_along_walks(emu, mma, ref_lib, n
         sess = emu.EmuSession(product(pb))
         assert sess.set_evaluator(form), (name, form)
         forms["form %d" % form] = sess
-    forms["mma"] = mma.MmaSession(product(pb))
+    forms["mma"] = mma(product(pb))
     cap = (1 << (39 - r.obj_bits)) - 1
     for what, start in starts.items():
         walks = [(PROBE, list(forms))]

@@ -3,11 +3,10 @@ tests/topics_ref/kao_topics_ref.c (the plain-C restatement of the search with to
 and the rows added to oracle.model's evaluation and HiGHS program.  Never part of the product."""
 import ctypes as C
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
 from oracle import model, ref
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -16,24 +15,11 @@ _DEPS = (_SRC, os.path.join(os.path.dirname(os.path.dirname(_HERE)), "oracle", "
 _lib = None
 
 
-def _build():
-    out_dir = os.path.join(_HERE, "_build")
-    try:
-        os.makedirs(out_dir, exist_ok=True)
-        if not os.access(out_dir, os.W_OK):
-            raise OSError
-    except OSError:
-        out_dir = tempfile.mkdtemp(prefix="kao_topics_ref_")
-    so = os.path.join(out_dir, "libkao_topics_ref.so")
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(d) for d in _DEPS):
-        subprocess.check_call(["gcc", "-O3", "-fopenmp", "-fPIC", "-std=c11", "-shared", "-o", so, _SRC])
-    return so
-
-
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(_build())
+        _lib = C.CDLL(native.shared_library(os.path.join(_HERE, "_build"), "libkao_topics_ref.so",
+                                            ["gcc", "-O3", "-fopenmp", "-fPIC", "-std=c11", "-shared", _SRC], _DEPS))
         _lib.kao_tref_search.restype = C.c_uint64
         _lib.kao_tref_topic_violation.restype = C.c_int64
         _lib.kao_ref_pack.restype = C.c_uint64
