@@ -137,7 +137,8 @@ template <class F> static int guarded(F &&f) noexcept
 // Device buffers are recycled across handles: kao_solve creates and destroys a session per call,
 // and cudaMalloc / cudaFree (which synchronises the device) would dominate short solves.
 namespace {
-struct DevPool {
+// Pinned host buffers (a search call's download staging) are recycled the same way: cudaMallocHost pins pages per call.
+template <bool kHost> struct BufPool {
     std::mutex mu;
     std::multimap<std::pair<int, size_t>, void *> free_;
     size_t held = 0;
@@ -149,18 +150,19 @@ struct DevPool {
             auto it = free_.find({dev, n});
             if (it != free_.end()) { *p = it->second; free_.erase(it); held -= n; return cudaSuccess; }
         }
-        return cudaMalloc(p, n);
+        return kHost ? cudaMallocHost(p, n) : cudaMalloc(p, n);
     }
     void put(int dev, void *p, size_t n)
     {
         n = (n + 255) & ~size_t(255);
         std::lock_guard<std::mutex> g(mu);
-        if (held + n > (size_t(1) << 30)) { cudaFree(p); return; }
+        if (held + n > (size_t(1) << 30)) { kHost ? cudaFreeHost(p) : cudaFree(p); return; }
         free_.insert({{dev, n}, p});
         held += n;
     }
 };
-DevPool g_pool;
+BufPool<false> g_pool;
+BufPool<true> g_host_pool;
 
 // a temporary device buffer that is freed on every path out of the scope that owns it
 template <class T> struct DevTmp {
@@ -186,6 +188,7 @@ constexpr size_t kBarBytes = 32;   // d_bar: [0] grid barrier, [1] release, [2] 
 
 struct kao_handle {
     std::vector<std::pair<void *, size_t>> owned;   // device buffers to hand back to the pool
+    std::vector<std::pair<void *, size_t>> owned_host;   // pinned host buffers to hand back to theirs
     HostModel hm;               // layout, tables, host copy of problem data
     int device = 0;
     int sms = 0;
@@ -206,7 +209,8 @@ struct kao_handle {
     Consts *d_consts = nullptr; unsigned long long *d_key = nullptr; unsigned long long *d_keys = nullptr;
     size_t keys_cap = 0;
     long long *d_vo = nullptr;
-    unsigned int *d_bar = nullptr;          // kBarBytes, see above
+    unsigned int *d_bar = nullptr;          // kBarBytes, see above; the round keys d_keys follow it in the same buffer
+    void *h_stage = nullptr;                // pinned host copy of d_bar and d_keys (kBarBytes + 8 * keys_cap bytes)
     // cross-GPU exchange (kao_p2p_*, kao_solve with n_gpus > 1)
     Mailbox *d_mail = nullptr;              // own mailbox (plain cudaMalloc: exported through CUDA IPC / used by peers directly)
     Mailbox *peer_mail[kMaxPeers] = {};
@@ -399,6 +403,7 @@ static int destroy_impl(kao_handle *h)
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();                   // nothing of this session may still be running on a recycled buffer
     for (auto &b : h->owned) g_pool.put(h->device, b.first, b.second);
+    for (auto &b : h->owned_host) g_host_pool.put(h->device, b.first, b.second);
     for (int r = 0; r < kMaxPeers; ++r)
         if (h->peer_opened[r]) cudaIpcCloseMemHandle(h->peer_mail[r]);
     if (h->d_mail && !h->mail_pooled) cudaFree(h->d_mail);
@@ -416,6 +421,8 @@ struct HandleOwner {
     ~HandleOwner() { close(); }
     void close() { const std::string keep = g_err; destroy_impl(h); g_err = keep; h = nullptr; }
 };
+
+static int reserve_keys(kao_handle *h, uint32_t rounds);
 
 static int reset_impl(kao_handle *h)
 {
@@ -526,7 +533,7 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, const kao_re
     CUDA_TRY(dalloc(h, &h->d_nD, 16));
     CUDA_TRY(dalloc(h, &h->d_consts, sizeof(Consts)));
     CUDA_TRY(dalloc(h, &h->d_key, 16));
-    CUDA_TRY(dalloc(h, &h->d_bar, kBarBytes));
+    { const int rc = reserve_keys(h, 0); if (rc != KAO_OK) return rc; }
     CUDA_TRY(cudaMemset(h->d_nD, 0, 16));
     { const unsigned long long none[2] = {kKeyNone, kKeyNone}; CUDA_TRY(cudaMemcpy(h->d_key, none, 16, cudaMemcpyHostToDevice)); }
     if (m.dense) {
@@ -677,11 +684,19 @@ static int check_search_args(const kao_handle *h, uint32_t rounds, uint32_t roun
     return KAO_OK;
 }
 
+// d_bar and the round keys in one device buffer, mirrored by one pinned host buffer: a search call downloads both
+// with one copy
 static int reserve_keys(kao_handle *h, uint32_t rounds)
 {
     if (h->keys_cap < rounds || !h->d_keys) {
-        h->d_keys = nullptr;                   // the old buffer stays owned by the handle until destroy
-        CUDA_TRY(dalloc(h, &h->d_keys, (size_t)(rounds > 0 ? rounds : 1) * 8));
+        // the old buffers stay owned by the handle until destroy
+        const size_t bytes = kBarBytes + (size_t)(rounds > 0 ? rounds : 1) * 8;
+        CUDA_TRY(dalloc(h, &h->d_bar, bytes));
+        h->d_keys = reinterpret_cast<unsigned long long *>(h->d_bar + kBarBytes / 4);
+        void *v = nullptr;
+        CUDA_TRY(g_host_pool.get(h->device, &v, bytes));
+        h->owned_host.emplace_back(v, bytes);
+        h->h_stage = v;
         h->keys_cap = rounds;
     }
     if (rounds) {
@@ -704,10 +719,11 @@ static P2P solo_p2p(kao_handle *h, uint32_t idx_lo, uint32_t idx_hi)
 }
 
 // A search call on a session around launch_rounds(), which enqueues its (at least one) rounds into h->d_keys: event
-// timing, the displaced lists in HBM rebuilt once at the end for the per-round entry points, the keys downloaded.
+// timing, the displaced lists in HBM rebuilt once at the end for the per-round entry points (unless the search kernel
+// left them there), d_bar and the keys downloaded into h->h_stage with one copy and one synchronisation.
 template <class F>
 static int timed_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
-                        uint64_t *round_keys, double *device_ms, F &&launch_rounds)
+                        uint64_t *round_keys, double *device_ms, bool delta, F &&launch_rounds)
 {
     CUDA_TRY(cudaSetDevice(h->device));
     h->last_rounds = 0;
@@ -716,8 +732,11 @@ static int timed_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint
     CUDA_TRY(cudaEventRecord(h->ev0, 0));
     if (rounds) {
         if ((rc = launch_rounds()) != KAO_OK) return rc;
-        // the large path keeps the displaced lists in HBM current itself
-        if (!h->large) CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
+        // the large path and the column-major search kernels keep the displaced lists in HBM current themselves
+        const bool lists_current = h->large || (!delta && h->evaluator == KAO_EVAL_COLUMN_MAJOR);
+        if (!lists_current) CUDA_TRY(launch_apply(h, seed, first_round, round_size, h->d_keys, /*regen_only=*/1, 0));
+        CUDA_TRY(cudaMemcpyAsync(h->h_stage, h->d_bar, kBarBytes + (round_keys ? (size_t)rounds * 8 : 0),
+                                 cudaMemcpyDeviceToHost, 0));
     }
     CUDA_TRY(cudaEventRecord(h->ev1, 0));
     CUDA_TRY(cudaEventSynchronize(h->ev1));
@@ -727,7 +746,7 @@ static int timed_search(kao_handle *h, uint64_t seed, uint32_t first_round, uint
         *device_ms = ms;
     }
     if (round_keys && rounds)
-        CUDA_TRY(cudaMemcpy(round_keys, h->d_keys, (size_t)rounds * 8, cudaMemcpyDeviceToHost));
+        std::memcpy(round_keys, static_cast<const uint8_t *>(h->h_stage) + kBarBytes, (size_t)rounds * 8);
     return KAO_OK;
 }
 
@@ -737,7 +756,7 @@ static int search_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint3
     if (!h) return fail(KAO_E_ARG, "null handle");
     int rc = check_search_args(h, rounds, round_size, delta);
     if (rc != KAO_OK) return rc;
-    rc = timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, [&]() -> int {
+    rc = timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, delta, [&]() -> int {
         // all rounds in one cooperative launch; the HBM base is kept current by CTA 0
         CUDA_TRY(cudaMemsetAsync(h->d_bar, 0, kBarBytes, 0));
         CUDA_TRY(launch_persistent(h, PersistArgs{seed, first_round, rounds, round_size, h->d_keys, h->d_bar, 0,
@@ -745,8 +764,8 @@ static int search_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint3
         return KAO_OK;
     });
     if (rc != KAO_OK || !rounds) return rc;
-    unsigned int st[4] = {0, 0, 0, 0};
-    CUDA_TRY(cudaMemcpy(st, h->d_bar, 16, cudaMemcpyDeviceToHost));
+    unsigned int st[4];
+    std::memcpy(st, h->h_stage, sizeof st);
     if (st[2]) return fail(KAO_E_CUDA, "search kernel timed out at a grid barrier");
     h->last_rounds = st[3];
     return KAO_OK;
@@ -850,7 +869,7 @@ static int sharded_impl(kao_handle *h, uint64_t seed, uint32_t first_round, uint
     const uint32_t lo = rank * base + ((uint32_t)rank < extra ? rank : extra);
     const uint32_t hi = lo + base + ((uint32_t)rank < extra ? 1 : 0);
     // one cooperative launch per kMailRounds rounds: the mailbox bank alternates from launch to launch
-    return timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, [&]() -> int {
+    return timed_search(h, seed, first_round, rounds, round_size, round_keys, device_ms, delta, [&]() -> int {
         unsigned long long best = kKeyNone;                         // early-stop state, carried from launch to launch
         uint32_t stall = 0;
         for (uint32_t done = 0; done < rounds; done += kMailRounds) {

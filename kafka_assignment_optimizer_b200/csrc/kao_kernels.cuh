@@ -74,8 +74,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
 #if defined(KAO_PHASE_CLOCKS)
 // per (CTA, warp, round): summed cycles of generate + park and of eval_batch_mma, the batches, and the stamps at the
 // round's start, after the warp's last batch, after the CTA reduce, the grid barrier, the winner's patch and rebuild_lists;
-// warps 1 .. of a sorted-batch schedule: after they sorted the next round's candidates (in the grid barrier's time)
-enum PhaseSlot { kPhGen, kPhEval, kPhBatches, kPhStart, kPhBatchesEnd, kPhReduce, kPhBarrier, kPhApply, kPhRebuild, kPhList, kPhSlots };
+// warps 1 .. of a sorted-batch schedule: after they sorted the next round's candidates (in the grid barrier's time).
+// The record of round 0 also holds the launch's ends: the SM clock and the global timer at the kernel's entry and after
+// its last round, so that the prologue and the tail are accounted for and the cycles convert to wall time.
+enum PhaseSlot { kPhGen, kPhEval, kPhBatches, kPhStart, kPhBatchesEnd, kPhReduce, kPhBarrier, kPhApply, kPhRebuild, kPhList,
+                 kPhEntry, kPhExit, kPhEntryNs, kPhExitNs, kPhSlots };
 constexpr int kPhaseWarps = 32, kPhaseRounds = 64;
 static __device__ unsigned long long *kao_phase_buf;
 __device__ __forceinline__ unsigned long long *phase_rec(int warp, uint32_t t)
@@ -106,20 +109,52 @@ __device__ __forceinline__ void build_oh_plane(uint32_t *s_bits, const uint8_t *
 
 // Column-major evaluator (kao_device_t.cuh): the two transposed planes and the term planes of the objective
 // are gathered once per launch from the staged row-major base (2 * W words per partition at off_sw, the term
-// planes at off_z; kS: and the shortfall planes of the tensor-core form behind the rack-field planes).
+// planes at off_z; kS: and the shortfall planes of the tensor-core form behind the rack-field planes).  A warp builds
+// whole words: lane b reads the row of partition 32 w + b once, and every plane word of w is one ballot over the lanes,
+// the same bits t_gather / z_gather / a_gather / s_gather form one partition at a time (lanes beyond Ppad, and for
+// the term and shortfall planes beyond P, give 0 as those stop there).  Lane j stores the word of plane j, or of slot
+// j + 32 t.
 template <int W, int THREADS, bool kS = false>
 __device__ __forceinline__ void build_t_planes(const Params &d, uint32_t *T, uint32_t *Z, const uint32_t *s_bits, const uint8_t *s_leader)
 {
-    constexpr int NSL = 32 * W;
-    const int nW = t_words(d.Ppad), total = kTPlanes * NSL * nW;
-    for (int o = threadIdx.x; o < total; o += THREADS) {
-        const int w = o % nW, s = (o / nW) % NSL, q = o / (nW * NSL);
-        T[t_word(q, s, w, nW, NSL)] = t_gather<W>(q, s, w, s_bits, s_leader, d.Ppad);
+    constexpr int NSL = 32 * W, kWarps = THREADS / 32;
+    constexpr int kRowPlanes = kZPlanes + kAPlanes<W>() + (kS ? kSPlanes : 0);
+    static_assert(kRowPlanes <= 32, "one row plane per lane");
+    const int nW = t_words(d.Ppad), lane = threadIdx.x & 31;
+    for (int w = threadIdx.x >> 5; w < nW; w += kWarps) {
+        const int p = 32 * w + lane;
+        const bool in_pad = p < d.Ppad, in_p = p < d.P;
+        uint32_t row[W];
+#pragma unroll
+        for (int t = 0; t < W; ++t) row[t] = in_pad ? s_bits[(size_t)t * d.Ppad + p] : 0u;
+        const int ld = in_pad ? (int)s_leader[p] : -1;
+#pragma unroll
+        for (int t = 0; t < W; ++t) {
+            uint32_t t0 = 0, t1 = 0;
+#pragma unroll
+            for (int b = 0; b < 32; ++b) {
+                const bool has = (row[t] >> b) & 1u;
+                const uint32_t h = __ballot_sync(0xFFFFFFFFu, has), l = __ballot_sync(0xFFFFFFFFu, has && ld == 32 * t + b);
+                if (lane == b) { t0 = h; t1 = l; }
+            }
+            T[t_word(0, 32 * t + lane, w, nW, NSL)] = t0;
+            T[t_word(1, 32 * t + lane, w, nW, NSL)] = t1;
+        }
+        int n = 0;
+#pragma unroll
+        for (int t = 0; t < W; ++t) n += __popc(row[t]);
+        uint32_t mine = 0;
+#pragma unroll
+        for (int j = 0; j < kRowPlanes; ++j) {
+            bool on;
+            if (j < kZPlanes) on = in_p && z_term_holds<W>(d, j, p, row, (uint32_t)ld);
+            else if (j < kZPlanes + kAPlanes<W>()) { const int b = j - kZPlanes; on = ((row[b >> 2] >> (8 * (b & 3))) & 0xFFu) != 0u; }
+            else on = in_p && ((max(d.RF - n, 0) >> (j - kZPlanes - kAPlanes<W>())) & 1);
+            const uint32_t v = __ballot_sync(0xFFFFFFFFu, on);
+            if (lane == j) mine = v;
+        }
+        if (lane < kRowPlanes) Z[(size_t)lane * nW + w] = mine;
     }
-    for (int o = threadIdx.x; o < kZPlanes * nW; o += THREADS) Z[o] = z_gather<W>(d, o / nW, o % nW, s_bits, s_leader);
-    for (int o = threadIdx.x; o < kAPlanes<W>() * nW; o += THREADS) Z[kZPlanes * nW + o] = a_gather<W>(o / nW, o % nW, s_bits, d.Ppad);
-    if constexpr (kS)
-        for (int o = threadIdx.x; o < kSPlanes * nW; o += THREADS) Z[(kZPlanes + kAPlanes<W>()) * nW + o] = s_gather<W>(d, o / nW, o % nW, s_bits);
     __syncthreads();
 }
 
@@ -484,6 +519,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
     const uint32_t obj_words = (!kObjShared || Cfg::kTrans) ? 0u : (Cfg::kObj > 0 ? (uint32_t)Cfg::kObj * W : (uint32_t)d.nentries);
     uint32_t *s_z = reinterpret_cast<uint32_t *>(smem + plan.off_z);
 
+    KAO_PHASE(const unsigned long long ph_entry = clock64(), ph_entry_ns = global_ns();)
     if (tid == 0) mbar_init(s_bar, 1);
     __syncthreads();
     if (tid == 0) {
@@ -545,7 +581,8 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         unsigned long long best = kKeyNone;
         KAO_PHASE(unsigned long long *ph = (lane == 0 && t < kPhaseRounds) ? phase_rec(warp, t) : nullptr;
                   unsigned long long ph_gen = 0, ph_eval = 0, ph_n = 0;
-                  if (ph) ph[kPhStart] = clock64();)
+                  if (ph) ph[kPhStart] = clock64();
+                  if (ph && t == 0) { ph[kPhEntry] = ph_entry; ph[kPhEntryNs] = ph_entry_ns; })
         if constexpr (kDelta) {
             // ---- delta mode: totals of the base once per round, then one THREAD per candidate
             const RoundTables rt = round_tables(smem, plan);
@@ -893,6 +930,17 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         if (s_red[kWarps]) break;
 #endif
     }
+    if constexpr (Cfg::kTrans) {
+        // the displaced lists of the base the search ended on, for the per-round entry points (kao_round_apply) that
+        // read them from HBM: CTA 0 stores its shared-memory copy, which rebuild_lists made from the same base
+        if (blockIdx.x == 0) {
+            const int nD = s_counts[0], nL = s_counts[1];
+            for (int i = tid; i < nD; i += THREADS) d.D[i] = s_D[i];
+            for (int i = tid; i < nL; i += THREADS) d.DL[i] = s_DL[i];
+            if (tid == 0) { d.nD[0] = nD; d.nD[1] = nL; }
+        }
+    }
+    KAO_PHASE(if (lane == 0 && rounds > 0) { unsigned long long *ph0 = phase_rec(warp, 0); ph0[kPhExit] = clock64(); ph0[kPhExitNs] = global_ns(); })
 }
 
 // ------------------------------------------------------------------------------------------
