@@ -314,18 +314,17 @@ int kao_set_patience(kao_handle *h, uint32_t rounds_without_improvement);
 #define KAO_EVAL_ROW_MAJOR 0
 #define KAO_EVAL_COLUMN_MAJOR 1
 int kao_set_evaluator(kao_handle *h, int32_t evaluator);
-/* Schedule of the column-major evaluator: the same arithmetic, laid out differently in time.  sync: how
- * the warps of a CTA meet before an evaluation and how the column loop is laid out (0 block barrier, 1 warp only with
- * the loop fully unrolled, 2 warp only with the loop kept a loop, 4 that loop unrolled by four); pop: one hex digit per
- * popcount stream (column totals in the low digit, leader totals in the next): 0 a POPC per word, 1 three per
- * four words, 2 two, 3 one (carry-save adders do the rest); a third digit 1 (pop 0x100) forms every sum on the
- * tensor cores instead, one binary MMA over a batch of 32 candidates (kao_device_mma.cuh), and 2 (pop 0x200) does so
- * with a generator whose later operations share their steps across link kinds (fewer divergent paths per warp), and
- * 3 (pop 0x300) does that with every CTA's candidates of a round sorted by the class of their control word first, so
- * that the 32 candidates of a batch mostly take one generator body, and scores two candidates per instruction in its
- * MMA epilogue (16 x 2 halfword pairs); a fourth digit 1 (pop 0x1300) keeps that epilogue in 32 bits per candidate;
- * threads per CTA: 512 .. 1024.  Only the six combinations built into the library are accepted (KAO_E_ARG otherwise);
- * the default (1, 0x300, 512) is the fastest one measured on an H100 (config 3; (4, 0x22, 1024) is the fastest popcount one).  Results never depend on it.  The environment variable
+/* Schedule of the column-major evaluator: the same arithmetic, laid out differently in time.  Two are built:
+ *   (1, 0x300, 512)   the default: every sum on the tensor cores, one binary MMA over a batch of 32 candidates
+ *                     (kao_device_mma.cuh), with every CTA's candidates of a round sorted by the class of their control
+ *                     word first, so that the 32 candidates of a batch mostly take one generator body, a generator whose
+ *                     later operations share their steps across link kinds, and an MMA epilogue that scores two
+ *                     candidates per instruction (16 x 2 halfword pairs); 512 threads per CTA
+ *   (4, 0x22, 1024)   one warp per candidate: the column loop unrolled by four (sync 4) and, in each popcount stream
+ *                     (column totals in the low hex digit of pop, leader totals in the next), two POPC per four words
+ *                     with carry-save adders doing the rest; 1024 threads per CTA
+ * Any other (sync, pop, threads) is refused (KAO_E_ARG).  The default is the fastest measured on an H100 (config 3;
+ * (4, 0x22, 1024) is the fastest popcount one).  Results never depend on it.  The environment variable
  * KAO_SCHEDULE="sync,pop(hex),threads" sets it for every session (and kao_solve); KAO_EVALUATOR=row forces
  * the row-major evaluator. */
 int kao_set_schedule(kao_handle *h, int32_t sync, int32_t pop, int32_t threads);

@@ -1,5 +1,5 @@
-// kao_device_mma.cuh — the column-major evaluator with its sums on the tensor cores (schedules with pop digit 2 = 1,
-// kao_device_t.cuh: EvalCfgT::kSums).
+// kao_device_mma.cuh — the column-major evaluator with its sums on the tensor cores (schedule pop 0x300,
+// kao_device_t.cuh: EvalCfgT).
 //
 // Every sum the column-major evaluator forms is a count of partitions p that hold in a base plane AND are scored
 // for the candidate.  For the 32 candidates c of a warp's batch these counts are one binary matrix product
@@ -50,7 +50,7 @@ inline void bmma_and_popc(int (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint
 #endif
 
 // ------------------------------------------------------------------------------------------
-// 16 x 2 SIMD for the packed epilogue (sorted-batch schedules): per-halfword unsigned max / min, SASS VIMNMX.U16x2,
+// 16 x 2 SIMD for the packed epilogue: per-halfword unsigned max / min, SASS VIMNMX.U16x2,
 // one instruction for two candidates.  The host build (test emulation) restates the CUDA semantics: each halfword of
 // the result is the max / min of the operands' halfwords, no carry or borrow between the halves.
 // ------------------------------------------------------------------------------------------
@@ -163,7 +163,7 @@ __device__ __forceinline__ int reduce_scatter8(int (&v)[8], int lane)
 }
 
 // ------------------------------------------------------------------------------------------
-// Sorted batches (schedules with pop digit 2 = 3).  The 32 lanes of a batch run the union of their candidates'
+// Sorted batches.  The 32 lanes of a batch run the union of their candidates'
 // generator bodies, and every branch of that union is chosen by the candidate's control word (docs/MODEL.md §5),
 // which depends on (seed, round, index) alone, not on the base.  So a CTA sorts its candidates of a round by the
 // class below before the round starts, and a batch takes 32 neighbours of that order: mostly one body.  The class:
@@ -265,7 +265,7 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     int v[8], o[8], rpen[2] = {0, 0};
 #pragma unroll
     for (int e = 0; e < 8; ++e) v[e] = o[e] = 0;
-    // Packed epilogue (Cfg::kPacked: pop 0x300; 0x1300 keeps the 32-bit form below): d0 / d1 of a lane are candidates 2 t and 2 t + 1 of one slot row, so the pair
+    // Packed epilogue: d0 / d1 of a lane are candidates 2 t and 2 t + 1 of one slot row, so the pair
     // travels as one register x = x0 | x1 << 16 (PRMT) and its delta bytes are spread into the two halves.  Every
     // column total is 0 <= c <= P <= 8,160, and with the bounds clamped to lo' = min(lo, P), hi' = min(hi, P)
     //     max(c - hi, 0) + max(lo - c, 0) = max(c, hi') + max(c, lo') - c  - hi' + (lo - lo')        (c <= P)
@@ -289,50 +289,29 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
         const int s = 16 * mt + lrow;
         tile(T + (size_t)(0 * NSL + s) * nW, swz ? 4 * (s & 7) : 0);
         int rk[8];
-        if constexpr (Cfg::kPacked) {
-            // per half and slot: 2 D + the C3 terms = max(c, hi') + max(c, lo') + D - delta, in 2 D .. 3 P; two slots
-            // <= 6 P = 48,960
-            uint32_t r[4] = {0u, 0u, 0u, 0u};
+        // per half and slot: 2 D + the C3 terms = max(c, hi') + max(c, lo') + D - delta, in 2 D .. 3 P; two slots
+        // <= 6 P = 48,960
+        uint32_t r[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int sl = 16 * mt + 8 * h + g;
-                uint32_t lo2, hi2;
-                bounds16x2(cs->bnd_rep[sl], PP, lo2, hi2);
-                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
-                const uint32_t nx = nb.x & 0x0F0F0F0Fu, ny = nb.y & 0x0F0F0F0Fu;
+        for (int h = 0; h < 2; ++h) {
+            const int sl = 16 * mt + 8 * h + g;
+            uint32_t lo2, hi2;
+            bounds16x2(cs->bnd_rep[sl], PP, lo2, hi2);
+            const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+            const uint32_t nx = nb.x & 0x0F0F0F0Fu, ny = nb.y & 0x0F0F0F0Fu;
 #pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    const uint32_t d2 = pair(nt, h), n2 = spread(nx, ny, nt), c2 = d2 + n2;
-                    r[nt] += vmax16x2(c2, hi2) + vmax16x2(c2, lo2) + d2 - n2;
-                    rk[4 * h + nt] = (int)c2;                       // c <= P < 8192: a rack's 8 slots stay below 2^16
-                }
-            }
-            widen(r);
-        } else {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int sl = 16 * mt + 8 * h + g;
-                const uint32_t b = cs->bnd_rep[sl];
-                const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
-                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                    for (int jj = 0; jj < 2; ++jj) {
-                        const int e = 2 * nt + jj;
-                        const int dd = acc[nt][2 * h + jj];
-                        const int c = dd + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3))) & 15u);
-                        v[e] += 2 * dd + max(c - hi, 0) + max(lo - c, 0);
-                        if (jj == 0) rk[4 * h + nt] = c;
-                        else rk[4 * h + nt] |= c << 16;         // c <= P < 8192: a rack's 8 slots stay below 2^16
-                    }
+            for (int nt = 0; nt < 4; ++nt) {
+                const uint32_t d2 = pair(nt, h), n2 = spread(nx, ny, nt), c2 = d2 + n2;
+                r[nt] += vmax16x2(c2, hi2) + vmax16x2(c2, lo2) + d2 - n2;
+                rk[4 * h + nt] = (int)c2;                       // c <= P < 8192: a rack's 8 slots stay below 2^16
             }
         }
+        widen(r);
         // rack totals: the 8 slots of a rack are the 8 lane groups; lane (g, t) gets rack 2 mt + (g >> 2) of candidates
         // 8 (g & 3) + 2 t + jj
         const int pk = reduce_scatter8(rk, lane);
-        const int r = 2 * mt + (g >> 2);
-        const int lo = r < d.R ? cs->rack_lo[r] : 0, hi = r < d.R ? cs->rack_hi[r] : 0x7FFFFFFF;
+        const int rack = 2 * mt + (g >> 2);
+        const int lo = rack < d.R ? cs->rack_lo[rack] : 0, hi = rack < d.R ? cs->rack_hi[rack] : 0x7FFFFFFF;
         const int t0 = pk & 0xFFFF, t1 = (int)((uint32_t)pk >> 16);
         rpen[0] += max(t0 - hi, 0) + max(lo - t0, 0);
         rpen[1] += max(t1 - hi, 0) + max(lo - t1, 0);
@@ -342,48 +321,28 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     for (int mt = 0; mt < 2 * W; ++mt) {
         const int s = 16 * mt + lrow;
         tile(T + (size_t)(1 * NSL + s) * nW, swz ? 4 * (s & 7) : 0);
-        if constexpr (Cfg::kPacked) {
-            // per half and slot: the C4 terms - l = max(l, hi') + max(l, lo') - 2 l, in 0 .. 2 P; two slots <= 4 P = 32,640
-            uint32_t m[4] = {0u, 0u, 0u, 0u}, ls[4] = {0u, 0u, 0u, 0u}, r[4];
+        // per half and slot: the C4 terms - l = max(l, hi') + max(l, lo') - 2 l, in 0 .. 2 P; two slots <= 4 P = 32,640
+        uint32_t m[4] = {0u, 0u, 0u, 0u}, ls[4] = {0u, 0u, 0u, 0u}, r[4];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int sl = 16 * mt + 8 * h + g;
-                uint32_t lo2, hi2;
-                bounds16x2(cs->bnd_ldr[sl], PP, lo2, hi2);
-                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
-                const uint32_t nx = (nb.x >> 4) & 0x0F0F0F0Fu, ny = (nb.y >> 4) & 0x0F0F0F0Fu;
+        for (int h = 0; h < 2; ++h) {
+            const int sl = 16 * mt + 8 * h + g;
+            uint32_t lo2, hi2;
+            bounds16x2(cs->bnd_ldr[sl], PP, lo2, hi2);
+            const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
+            const uint32_t nx = (nb.x >> 4) & 0x0F0F0F0Fu, ny = (nb.y >> 4) & 0x0F0F0F0Fu;
 #pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    const uint32_t l2 = pair(nt, h) + spread(nx, ny, nt);
-                    m[nt] += vmax16x2(l2, hi2) + vmax16x2(l2, lo2);
-                    ls[nt] += l2;
-                }
-            }
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt) r[nt] = m[nt] - 2u * ls[nt];
-            widen(r);
-        } else {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int sl = 16 * mt + 8 * h + g;
-                const uint32_t b = cs->bnd_ldr[sl];
-                const int lo = (int)(b & 0xFFFFu), hi = (int)(b >> 16);
-                const uint2 nb = *reinterpret_cast<const uint2 *>(cols + 32 * sl);
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                    for (int jj = 0; jj < 2; ++jj) {
-                        const int e = 2 * nt + jj;
-                        const int l = acc[nt][2 * h + jj] + (int)(((e < 4 ? nb.x : nb.y) >> (8 * (e & 3) + 4)) & 15u);
-                        v[e] += max(l - hi, 0) + max(lo - l, 0) - l;
-                    }
+            for (int nt = 0; nt < 4; ++nt) {
+                const uint32_t l2 = pair(nt, h) + spread(nx, ny, nt);
+                m[nt] += vmax16x2(l2, hi2) + vmax16x2(l2, lo2);
+                ls[nt] += l2;
             }
         }
-    }
-    if constexpr (Cfg::kPacked) {
 #pragma unroll
-        for (int nt = 0; nt < 4; ++nt) v[2 * nt] = (int)((uint32_t)v[2 * nt] - ((uint32_t)v[2 * nt + 1] << 16));
+        for (int nt = 0; nt < 4; ++nt) r[nt] = m[nt] - 2u * ls[nt];
+        widen(r);
     }
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) v[2 * nt] = (int)((uint32_t)v[2 * nt] - ((uint32_t)v[2 * nt + 1] << 16));
     // ---- term planes (objective), rack-field planes (- z) and shortfall planes (+ 2 * 2^k): rows Z[0..8 + 4 W + 4),
     // one tile at W = 1, two at W = 2 (the second one's rows beyond the shortfall planes repeat them and weigh nothing)
     constexpr int kZRows = kZPlanes + 4 * W + kSPlanes;
@@ -415,12 +374,10 @@ __device__ __forceinline__ void eval_batch_mma(const Params &d, const Consts *cs
     const uint4 h = *reinterpret_cast<const uint4 *>(batch + mma_lane_candidate(lane) * kBatchHdr);
     viol_out = viol + (int)h.z + d.P - d.RF * (d.P - (int)(h.y >> 16));
     obj_out = obj + (int)h.w;
-    if constexpr (Cfg::kPacked) {                                  // the clamp's constant, over every slot of both tables
-        int k = 0;
+    int k = 0;                                                      // the clamp's constant, over every slot of both tables
 #pragma unroll
-        for (int sl = lane; sl < NSL; sl += 32) k += bounds16x2_rest(cs->bnd_rep[sl], PP) + bounds16x2_rest(cs->bnd_ldr[sl], PP);
-        viol_out += __reduce_add_sync(0xFFFFFFFFu, k);
-    }
+    for (int sl = lane; sl < NSL; sl += 32) k += bounds16x2_rest(cs->bnd_rep[sl], PP) + bounds16x2_rest(cs->bnd_ldr[sl], PP);
+    viol_out += __reduce_add_sync(0xFFFFFFFFu, k);
 }
 
 }  // namespace kao

@@ -36,28 +36,24 @@ namespace kao {
 
 // kNW: partition words per slot fixed at compile time (32 = 1024 padded partitions, the headline
 // shape: every shared-memory offset of the evaluator is then an immediate), 0 = read at run time.
-// The other parameters are SCHEDULES of the same arithmetic (kao_set_schedule; results identical):
-//   kSync      how the warps of a CTA meet before an evaluation: 0 block barrier (all warps walk the
-//              evaluator together), 1 warp only (one warp's generator overlaps another's evaluation), 2 warp only
-//              with the column loop kept a loop (a third less evaluator code for the instruction cache), 3 / 4 that loop
-//              unrolled by 2 / 4
-//   kPop       how the two popcount streams (column totals, leader totals) trade POPC (XU pipe, 8 cycles
-//              a warp) for carry-save LOP3 (ALU pipe, 2 cycles): one hex digit per stream, 0 = a POPC per
-//              word, 1 = three per four words, 2 = two, 3 = one (Harley-Seal accumulators carried across
-//              the whole column)
-//              a third hex digit picks where the sums are formed: 0 = the popcount streams above, 1 = on the tensor
-//              cores, a binary MMA over a batch of 32 candidates (kao_device_mma.cuh; the two low digits and kSync
-//              then play no part)
-//              with the third digit 3 the MMA epilogue scores two candidates per instruction in 16 x 2 halfword pairs
-//              (kao_device_mma.cuh, eval_batch_mma); a fourth hex digit 1 keeps it in 32 bits per candidate
+// The other parameters are SCHEDULES of the same arithmetic (kao_set_schedule; results identical).  The search
+// kernels are built in two (kao_kernels.cuh, KAO_FOR_SCHEDULES), as (kSync, kPop, kThreads):
+//   (1, 0x300, 512)    the default: every sum on the tensor cores, a binary MMA over a batch of 32 candidates taken from
+//                      the CTA's candidates sorted by class, whose epilogue scores two candidates per instruction in
+//                      16 x 2 halfword pairs (kao_device_mma.cuh, eval_batch_mma); kSync plays no part
+//   (4, 0x22, 1024)    the popcount streams of eval_candidate_t below, one candidate per warp at a time
+//   kSync      how eval_candidate_t lays out its column loop: below 2 unrolled in full where the word count is fixed
+//              (32 words), else kept a loop; 4 unrolled by 4
+//   kPop       0x300: the tensor-core form above.  Else how the two popcount streams (column totals, leader totals)
+//              trade POPC (XU pipe, 8 cycles a warp) for carry-save LOP3 (ALU pipe, 2 cycles): one hex digit per
+//              stream, 0 = a POPC per word, 1 = three per four words, 2 = two, 3 = one (Harley-Seal accumulators
+//              carried across the whole column)
 //   kThreads   threads per CTA (0 = threads_for<W>()); fewer threads = more registers per thread
 template <int W_, int kNW_ = 0, int kSync_ = 1, int kPop_ = 0x22, int kThreads_ = 0>
 struct EvalCfgT {
     static constexpr int W = W_, NPH = 5, kRack = 3, kObj = 3, kNW = kNW_;
     static constexpr int kSync = kSync_, kPop = kPop_, kThreads = kThreads_;
-    static constexpr int kSums = (kPop_ >> 8) & 15;
-    static constexpr bool kPacked = kSums == 3 && !((kPop_ >> 12) & 1);
-    static_assert(!((kPop_ >> 12) & 1) || kSums == 3, "the 32-bit epilogue digit applies to the sorted-batch body");
+    static constexpr bool kPacked = kPop_ == 0x300;     // the tensor-core form, with its packed epilogue
     static constexpr bool kTrans = true;
 };
 constexpr int kTPlanes = 2;
@@ -323,9 +319,6 @@ __device__ void eval_candidate_t(const Params &d, const uint32_t *Tp, int nW_rt,
     if constexpr (kNW == 32 && Cfg::kSync < 2) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) { uint4 c[W], o[W]; load(j, c, o); add(c, o); }
-    } else if constexpr (Cfg::kSync == 3) {          // nch is even (t_words rounds to whole groups of 8 words)
-#pragma unroll 2
-        for (int j = 0; j < nch; ++j) { uint4 c[W], o[W]; load(j, c, o); add(c, o); }
     } else if constexpr (Cfg::kSync == 4) {
 #pragma unroll 4
         for (int j = 0; j < nch; ++j) { uint4 c[W], o[W]; load(j, c, o); add(c, o); }

@@ -200,8 +200,8 @@ struct kao_handle {
     bool trans_ok = false;
     int evaluator = KAO_EVAL_ROW_MAJOR;
     SmemPlan plan_t{};
-    // schedule of the column-major evaluator (kao_set_schedule): barrier form, popcount compression per
-    // stream, threads per CTA.  Same results whatever the schedule.
+    // schedule of the column-major evaluator (kao_set_schedule): column-loop form, tensor cores or popcount
+    // compression per stream, threads per CTA.  Same results whatever the schedule.
     int sch_sync = KAO_SCHEDULE_DEFAULT_SYNC, sch_pop = KAO_SCHEDULE_DEFAULT_POP, sch_threads = KAO_SCHEDULE_DEFAULT_THREADS;
     // device buffers
     uint32_t *d_bits = nullptr; uint8_t *d_leader = nullptr; uint32_t *d_sw = nullptr;
@@ -291,7 +291,7 @@ template <bool kDelta> struct LaunchPersistent {
         // the column-major plan depends on the warps per CTA of the schedule (per-warp scratch) and, with sorted batches,
         // on the candidates of a CTA per round (the most any CTA takes: its warps' iterations)
         const uint32_t stride = (uint32_t)h->grid * (T / 32), share = a.pp.idx_hi - a.pp.idx_lo;
-        const uint32_t cands = cfg_sorted<Cfg>() ? (share + stride - 1) / stride * (T / 32) : 0;
+        const uint32_t cands = cfg_mma<Cfg>() ? (share + stride - 1) / stride * (T / 32) : 0;
         SmemPlan plan = Cfg::kTrans ? make_plan_t(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF, cfg_mma<Cfg>(), cands)
                         : (kDelta && Cfg::W > 2) ? make_plan_delta_wide(Cfg::W, h->hm.Ppad, T, h->hm.P, h->hm.RF) : h->plan;
         if (plan.total > 227u * 1024u) return cudaErrorInvalidConfiguration;

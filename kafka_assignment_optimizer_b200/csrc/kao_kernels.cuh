@@ -28,16 +28,11 @@ template <class Cfg> constexpr int cfg_threads()
     if constexpr (Cfg::kTrans) return Cfg::kThreads ? Cfg::kThreads : threads_for<Cfg::W>();
     else return threads_for<Cfg::W>();
 }
-// does a configuration form its sums on the tensor cores (column-major, kao_device_mma.cuh)
+// does a configuration form its sums on the tensor cores (column-major, kao_device_mma.cuh), in batches taken from the
+// CTA's candidates sorted by class (cand_class)
 template <class Cfg> __host__ __device__ constexpr bool cfg_mma()
 {
-    if constexpr (Cfg::kTrans) return Cfg::kSums >= 1;
-    else return false;
-}
-// does a configuration take its batches from the CTA's candidates sorted by class (kao_device_mma.cuh, cand_class)
-template <class Cfg> __host__ __device__ constexpr bool cfg_sorted()
-{
-    if constexpr (Cfg::kTrans) return Cfg::kSums == 3;
+    if constexpr (Cfg::kTrans) return Cfg::kPacked;
     else return false;
 }
 
@@ -558,8 +553,8 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
     const uint32_t first = pp.idx_lo + blockIdx.x * kWarps;
     const uint32_t iters = first < pp.idx_hi ? (pp.idx_hi - first + stride - 1) / stride : 0;
     // sorted batches: the CTA's candidates of a round sorted by class, behind the class histogram.  A share beyond the
-    // plan's list (rounds near KAO_MAX_ROUND_SIZE) walks its candidates unsorted, as the other schedules do
-    constexpr bool kSorted = cfg_sorted<Cfg>();
+    // plan's list (rounds near KAO_MAX_ROUND_SIZE) walks its candidates unsorted, every warp its own in index order
+    constexpr bool kSorted = cfg_mma<Cfg>();
     int *s_hist = reinterpret_cast<int *>(smem + plan.off_inv);
     uint32_t *s_list = reinterpret_cast<uint32_t *>(s_hist + kCandClasses);
     uint8_t *s_cls = reinterpret_cast<uint8_t *>(s_list + cand_list_cap(plan));
@@ -626,11 +621,10 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         } else if constexpr (cfg_mma<Cfg>()) {
             // ---- column-major evaluator, sums on the tensor cores (kao_device_mma.cuh): candidates are generated 32 at a
             // time, one per LANE, as below, then the warp evaluates all 32 together; lane (g, t) ends with the
-            // violation and objective of candidate mma_lane_candidate(lane) of the batch.  Pop digit 2 = 2: the later
-            // operations' link kinds share their steps (Gen kMerged), same candidates.  Pop digit 2 = 3: as 2, and the batches
-            // come from the CTA's candidates sorted by class (s_list), batch b of them to warp b mod kWarps, so that every
-            // warp takes a share of each class
-            Gen<W, true, true, Cfg::kSums >= 2> tg;        // compact code (row_kth keeps its loop), same candidates
+            // violation and objective of candidate mma_lane_candidate(lane) of the batch.  The later operations' link kinds
+            // share their steps (Gen kMerged), same candidates.  The batches come from the CTA's candidates sorted by class
+            // (s_list), batch b of them to warp b mod kWarps, so that every warp takes a share of each class
+            Gen<W, true, true, true> tg;        // compact code (row_kth keeps its loop), same candidates
             tg.bitsT = s_bits; tg.leader = s_leader; tg.cs = s_cs; tg.d = &d; tg.prow = nullptr; tg.lane = 0;
             tg.D = s_D; tg.DL = s_DL; tg.nD = s_counts[0]; tg.nL = s_counts[1];
             tg.T = s_sw; tg.tnW = t_words(d.Ppad); tg.t_leaders_valid = s_counts[2] == 0;    // "first holder of slot s": plane scan
@@ -731,7 +725,6 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
                 const uint32_t nb = iters - it0 < 32u ? iters - it0 : 32u;
                 for (uint32_t j = 0; j < nb; ++j) {
                     const uint32_t idx = first + warp + (it0 + j) * stride;
-                    if constexpr (Cfg::kSync == 0) __syncthreads();          // all warps walk the evaluator together
                     if (idx < pp.idx_hi) {
                         const uint32_t *slot = batch + j * BS;
                         const uint4 hdr = *reinterpret_cast<const uint4 *>(slot);
@@ -960,7 +953,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
 // Column-major kernels: X(sync, pop, threads) for every built schedule (kao_set_schedule); each is
 // instantiated for W = 1, 2 and for 32 partition words (compile-time offsets) / any word count.
 #define KAO_FOR_SCHEDULES(X) \
-    X(1, 0x300, 512) X(1, 0x1300, 512) X(1, 0x200, 512) X(1, 0x100, 512) X(4, 0x22, 1024) X(4, 0x22, 896)
+    X(1, 0x300, 512) X(4, 0x22, 1024)
 #define KAO_SCHEDULE_DEFAULT_SYNC 1
 #define KAO_SCHEDULE_DEFAULT_POP 0x300
 #define KAO_SCHEDULE_DEFAULT_THREADS 512

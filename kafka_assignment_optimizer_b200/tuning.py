@@ -1,9 +1,10 @@
 """Measuring the engine's full-evaluation variants on the GPU at hand.
 
 The engine has two full evaluators with bit-identical results (column-major: the default wherever the
-layout allows it, docs/MODEL.md §3.3; row-major: every layout) and builds the column-major one in a few
-*schedules* of the same arithmetic (include/kao.h, kao_set_schedule).  The library's default schedule is
-the one that was fastest on an H100 (config 3); nothing has to be tuned to get it.  `probe()` re-measures
+layout allows it, docs/MODEL.md §3.3; row-major: every layout) and builds the column-major one in two
+*schedules* of the same arithmetic, on the tensor cores and in popcount streams (include/kao.h,
+kao_set_schedule).  The library's default schedule is the one that was fastest on an H100 (config 3); nothing
+has to be tuned to get it.  `probe()` re-measures
 every built variant on the caller's problem — `python bench.py --probe-schedules` prints its lines — and
 checks that all of them return the row-major evaluator's round keys and final assignment.
 """
@@ -12,11 +13,10 @@ from __future__ import annotations
 import json
 
 # (sync, pop, threads) — the variants csrc/kao_kernels.cuh builds (KAO_FOR_SCHEDULES); the first is the default.
-# pop 0x100: the sums on the tensor cores (binary MMA, csrc/kao_device_mma.cuh); 0x200: the same with the merged generator;
-# 0x300: the same with each CTA's candidates sorted by class (control word) before a round, so a batch runs mostly one body,
-# and the MMA epilogue scoring two candidates per instruction in 16 x 2 halfword pairs; 0x1300: the same with the epilogue
-# in 32 bits per candidate
-SCHEDULES = [(1, 0x300, 512), (1, 0x1300, 512), (1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 1024), (4, 0x22, 896)]
+# pop 0x300: the sums on the tensor cores (binary MMA, csrc/kao_device_mma.cuh) over batches of each CTA's candidates
+# sorted by class (control word) before a round, so a batch runs mostly one body, with the MMA epilogue scoring two
+# candidates per instruction in 16 x 2 halfword pairs; 0x22: the popcount streams, two POPC per four words in each
+SCHEDULES = [(1, 0x300, 512), (4, 0x22, 1024)]
 DEFAULT_SCHEDULE = SCHEDULES[0]
 SCHEDULE_FIELDS = ("sync", "pop", "threads")
 

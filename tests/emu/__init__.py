@@ -138,8 +138,8 @@ def rows_charged_one_by_one():
 
 class MmaSession:
     """The calls the parity tests use, with every key from the batched tensor-core body (csrc/kao_device_mma.cuh) of
-    pop digit `pop`: 0x100, or 0x300 for the packed epilogue of the sorted-batch schedule.  Raises ValueError on a
-    layout the column-major evaluator does not cover."""
+    pop digit `pop`: 0x300, the default schedule's, with its packed epilogue.  Raises ValueError on any other pop
+    digit and on a layout the column-major evaluator does not cover."""
 
     def __init__(self, pb, pop):
         from kafka_assignment_optimizer_b200.optimizer import _CProblem

@@ -3,9 +3,9 @@
 // base, per-thread generator, row-major evaluator) plus the batched body, ldmatrix and the binary MMA restated by
 // mma_emu.hpp.  As one warp of the search kernel does it, 32 candidates are generated one per lane, parked in the
 // warp's batch and evaluated together; winners patch the transposed, term, rack-field and shortfall planes with
-// t_patch_row.  A session runs one pop digit: 0x100 (the unsorted schedules) or 0x300 (the sorted-batch schedule,
-// whose packed epilogue runs its 16 x 2 SIMD as the header's host restatement).  Its keys come in batches in index
-// order, so every shape and round size reaches the epilogue, or in the sorted batches of csrc/kao_kernels.cuh
+// t_patch_row.  The body is the default schedule's, pop 0x300, whose packed epilogue runs its 16 x 2 SIMD as the
+// header's host restatement.  Its keys come in batches in index order (as a CTA whose share exceeds its sorted list
+// walks them), so every shape and round size reaches the epilogue, or in the sorted batches of csrc/kao_kernels.cuh
 // (build_cand_list and the batch loop of search_persistent_kernel): every CTA sorts its share of a round by cand_class
 // and its warps generate, park and evaluate batches of 32 neighbours of that order.  tests/test_mma_emulation.py,
 // tests/test_packed_epilogue.py and tests/test_mma_sorted_batches.py check it against the oracle restatement.
@@ -16,11 +16,8 @@
 
 namespace {
 
-static_assert(EvalCfgT<1, 0, 1, 0x300>::kPacked && !EvalCfgT<1, 0, 1, 0x1300>::kPacked, "pop 0x300 is the packed epilogue");
-
 struct MmaEmu {
     Emu *e = nullptr;
-    int pop = 0x100;                     // pop digit of the evaluator: 0x100, or 0x300 for the packed epilogue
     std::vector<uint32_t> T, Z;          // transposed planes; term, rack-field and shortfall planes
 };
 
@@ -53,8 +50,8 @@ template <int W> Gen<W, true, true> make_gen(MmaEmu &x)
 
 // one batch of the search kernel: lane j < count (count <= 32) generates candidate idx[j], or idx0 + j when idx is
 // null, and the warp parks and evaluates the 32 together; out[j]: candidate j's key
-template <int W, int POP> void keys_batch(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t idx0, const uint32_t *idx,
-                                          uint32_t count, uint32_t round_size, unsigned long long *out)
+template <int W> void keys_batch(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t idx0, const uint32_t *idx,
+                                 uint32_t count, uint32_t round_size, unsigned long long *out)
 {
     Emu &e = *x.e;
     alignas(16) uint32_t batch[32 * batch_stride_words(W)];
@@ -74,19 +71,19 @@ template <int W, int POP> void keys_batch(MmaEmu &x, uint64_t seed, uint32_t rou
         mma_park_patch<W>(ps, rows, pviol, pobj, batch, lane);
         __syncwarp();
         int viol, obj;
-        if (e.nW == 32) eval_batch_mma<EvalCfgT<W, 32, 1, POP>>(e.prm, &e.cs, x.T.data(), e.nW, x.Z.data(), batch, lane, viol, obj);
-        else eval_batch_mma<EvalCfgT<W, 0, 1, POP>>(e.prm, &e.cs, x.T.data(), e.nW, x.Z.data(), batch, lane, viol, obj);
+        if (e.nW == 32) eval_batch_mma<EvalCfgT<W, 32, 1, 0x300>>(e.prm, &e.cs, x.T.data(), e.nW, x.Z.data(), batch, lane, viol, obj);
+        else eval_batch_mma<EvalCfgT<W, 0, 1, 0x300>>(e.prm, &e.cs, x.T.data(), e.nW, x.Z.data(), batch, lane, viol, obj);
         const uint32_t j = (uint32_t)mma_lane_candidate(lane);
         if (j < count) out[j] = pack_key(viol, obj, idx ? idx[j] : idx0 + j, e.prm.key_obj_bits);
     });
 }
 
 // candidates idx0 .. idx0 + count - 1 in batches of 32 in index order
-template <int W, int POP> void keys(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t idx0, uint32_t count, uint32_t round_size,
-                                    unsigned long long *out)
+template <int W> void keys(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t idx0, uint32_t count, uint32_t round_size,
+                           unsigned long long *out)
 {
     for (uint32_t i = 0; i < count; i += 32)
-        keys_batch<W, POP>(x, seed, round, idx0 + i, nullptr, std::min(32u, count - i), round_size, out + i);
+        keys_batch<W>(x, seed, round, idx0 + i, nullptr, std::min(32u, count - i), round_size, out + i);
 }
 
 // the winner becomes the base: every lane rewrites its words of the planes (t_patch_row with the shortfall planes),
@@ -122,12 +119,12 @@ template <int W> void apply(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t i
 }
 
 // whole rounds: argmin of the keys, the winner becomes the base (kao_search, one GPU, no early stop)
-template <int W, int POP> void search(MmaEmu &x, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
-                                      uint64_t *round_keys)
+template <int W> void search(MmaEmu &x, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size,
+                             uint64_t *round_keys)
 {
     std::vector<unsigned long long> all(round_size);
     for (uint32_t t = 0; t < rounds; ++t) {
-        keys<W, POP>(x, seed, first_round + t, 0, round_size, round_size, all.data());
+        keys<W>(x, seed, first_round + t, 0, round_size, round_size, all.data());
         unsigned long long best = kKeyNone;
         for (uint32_t i = 0; i < round_size; ++i) best = std::min(best, all[i]);
         if (round_keys) round_keys[t] = best;
@@ -138,7 +135,7 @@ template <int W, int POP> void search(MmaEmu &x, uint64_t seed, uint32_t first_r
 // CTA c of `grid` CTAs of `warps` warps takes first = idx_lo + c * warps, + stride, ... below idx_hi.  If that share
 // holds at most `cap` candidates it is sorted by cand_class (counting sort; the kernel's order within a class is
 // arbitrary, this one keeps the positions' order) and cut into batches of 32; else every warp walks its own candidates
-// in batches of 32 as the unsorted schedules do.  Returns the share in batch order; `bounds`: where each batch ends.
+// in batches of 32 in index order.  Returns the share in batch order; `bounds`: where each batch ends.
 std::vector<uint32_t> cta_batches(uint64_t seed, uint32_t round, uint32_t round_size, uint32_t idx_lo, uint32_t idx_hi,
                                   uint32_t grid, uint32_t warps, uint32_t cap, uint32_t cta, std::vector<uint32_t> &bounds)
 {
@@ -164,8 +161,8 @@ std::vector<uint32_t> cta_batches(uint64_t seed, uint32_t round, uint32_t round_
     return list;
 }
 
-template <int W, int POP> void sorted_keys(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t round_size, uint32_t idx_lo,
-                                           uint32_t idx_hi, uint32_t grid, uint32_t warps, uint32_t cap, unsigned long long *out)
+template <int W> void sorted_keys(MmaEmu &x, uint64_t seed, uint32_t round, uint32_t round_size, uint32_t idx_lo,
+                                  uint32_t idx_hi, uint32_t grid, uint32_t warps, uint32_t cap, unsigned long long *out)
 {
     unsigned long long k32[32];
     std::vector<uint32_t> bounds;
@@ -173,7 +170,7 @@ template <int W, int POP> void sorted_keys(MmaEmu &x, uint64_t seed, uint32_t ro
         const std::vector<uint32_t> list = cta_batches(seed, round, round_size, idx_lo, idx_hi, grid, warps, cap, c, bounds);
         for (size_t b = 0; b + 1 < bounds.size(); ++b) {
             const uint32_t count = bounds[b + 1] - bounds[b];
-            keys_batch<W, POP>(x, seed, round, 0, list.data() + bounds[b], count, round_size, k32);
+            keys_batch<W>(x, seed, round, 0, list.data() + bounds[b], count, round_size, k32);
             for (uint32_t j = 0; j < count; ++j) out[list[bounds[b] + j] - idx_lo] = k32[j];
         }
     }
@@ -183,21 +180,15 @@ template <int N> using Int = std::integral_constant<int, N>;
 
 template <class F> void with_w(MmaEmu &x, F f) { if (x.e->hm.W == 1) f(Int<1>{}); else f(Int<2>{}); }
 
-// f(W, POP) for the session's row width and pop digit
-template <class F> void with_w_pop(MmaEmu &x, F f)
-{
-    with_w(x, [&](auto w) { if (x.pop == 0x100) f(w, Int<0x100>{}); else f(w, Int<0x300>{}); });
-}
-
 }  // namespace
 
 extern "C" {
 
-// pop: 0x100 or 0x300 (the packed epilogue).  nullptr (kao_emu_last_error) unless the column-major evaluator covers
-// the layout
+// pop: the schedule's pop digit, 0x300 (the one tensor-core form built).  nullptr (kao_emu_last_error) unless the
+// column-major evaluator covers the layout
 void *kao_emu_tc_create(const kao_problem *pb, int32_t pop)
 {
-    if (pop != 0x100 && pop != 0x300) { g_err = "tensor-core evaluator: pop digit 0x100 or 0x300"; return nullptr; }
+    if (pop != 0x300) { g_err = "tensor-core evaluator: pop digit 0x300"; return nullptr; }
     Emu *e = static_cast<Emu *>(kao_emu_create(pb));
     if (!e) return nullptr;
     if (!e->trans_ok) {
@@ -207,7 +198,6 @@ void *kao_emu_tc_create(const kao_problem *pb, int32_t pop)
     }
     auto *x = new MmaEmu;
     x->e = e;
-    x->pop = pop;
     with_w(*x, [&](auto w) { build_planes<decltype(w)::value>(*x); });
     return x;
 }
@@ -237,9 +227,8 @@ void kao_emu_tc_candidate_keys(void *h, uint64_t seed, uint32_t round, uint32_t 
                                uint64_t *out)
 {
     auto &x = *static_cast<MmaEmu *>(h);
-    with_w_pop(x, [&](auto w, auto pop) {
-        keys<decltype(w)::value, decltype(pop)::value>(x, seed, round, idx_begin, count, round_size,
-                                                       reinterpret_cast<unsigned long long *>(out));
+    with_w(x, [&](auto w) {
+        keys<decltype(w)::value>(x, seed, round, idx_begin, count, round_size, reinterpret_cast<unsigned long long *>(out));
     });
 }
 
@@ -248,9 +237,9 @@ void kao_emu_tc_sorted_keys(void *h, uint64_t seed, uint32_t round, uint32_t rou
                             uint32_t grid, uint32_t warps, uint32_t cap, uint64_t *out)
 {
     auto &x = *static_cast<MmaEmu *>(h);
-    with_w_pop(x, [&](auto w, auto pop) {
-        sorted_keys<decltype(w)::value, decltype(pop)::value>(x, seed, round, round_size, idx_lo, idx_hi, grid, warps, cap,
-                                                              reinterpret_cast<unsigned long long *>(out));
+    with_w(x, [&](auto w) {
+        sorted_keys<decltype(w)::value>(x, seed, round, round_size, idx_lo, idx_hi, grid, warps, cap,
+                                        reinterpret_cast<unsigned long long *>(out));
     });
 }
 
@@ -278,9 +267,7 @@ int kao_emu_tc_check_state(void *h, int64_t *at)
 void kao_emu_tc_search(void *h, uint64_t seed, uint32_t first_round, uint32_t rounds, uint32_t round_size, uint64_t *round_keys)
 {
     auto &x = *static_cast<MmaEmu *>(h);
-    with_w_pop(x, [&](auto w, auto pop) {
-        search<decltype(w)::value, decltype(pop)::value>(x, seed, first_round, rounds, round_size, round_keys);
-    });
+    with_w(x, [&](auto w) { search<decltype(w)::value>(x, seed, first_round, rounds, round_size, round_keys); });
 }
 
 // CTA cta's candidates in the order its warps generate them, their classes and where each batch ends; 1 if sorted

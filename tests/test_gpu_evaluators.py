@@ -149,7 +149,7 @@ def test_unsupported_layouts_are_refused():
 
 
 def test_every_schedule_gives_the_same_keys():
-    """kao_set_schedule: barrier form, popcount compression per stream, threads per CTA — same results,
+    """kao_set_schedule: tensor cores or popcount streams, column loop, threads per CTA — same results,
     on the headline shape (32 partition words, compile-time offsets) and on a small one-word shape."""
     from kafka_assignment_optimizer_b200 import tuning
 
@@ -169,6 +169,8 @@ def test_every_schedule_gives_the_same_keys():
             sess.close()
     sess = kao.Session(product(SHAPES["cfg2"]()))
     assert not sess.set_schedule(1, 0x12345, 768) and not sess.set_schedule(2, 0x11111, 768)   # only what is built
+    for retired in [(1, 0x1300, 512), (1, 0x200, 512), (1, 0x100, 512), (4, 0x22, 896)]:        # superseded, no longer built
+        assert not sess.set_schedule(*retired), retired
     sess.close()
 
 

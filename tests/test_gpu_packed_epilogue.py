@@ -1,7 +1,7 @@
 """The default tensor-core schedule (1, 0x300, 512) scores two candidates per instruction in its MMA epilogue (16 x 2
-halfword pairs, csrc/kao_device_mma.cuh); (1, 0x1300, 512) is the same body with the epilogue in 32 bits.  Keys,
-trajectories and bases must be the restatement's, bit for bit, with bounds far above the column totals, bounds of 0, at
-the largest column-major row count, and in a round too large for the sorted list."""
+halfword pairs, csrc/kao_device_mma.cuh).  Keys, trajectories and bases must be the restatement's, bit for bit, with
+bounds far above the column totals, bounds of 0, at the largest column-major row count, and, against the popcount
+schedule (4, 0x22, 1024), in a round too large for the sorted list."""
 import numpy as np
 import pytest
 
@@ -13,7 +13,7 @@ from test_packed_epilogue import with_extreme_bounds, with_random_bounds
 
 pytestmark = pytest.mark.gpu
 PACKED = (1, 0x300, 512)
-WIDE = (1, 0x1300, 512)
+POPCOUNT = (4, 0x22, 1024)
 SEED = 0xC0FFEE
 SHAPES_BOUNDS = {
     "cfg3_extreme": lambda: with_extreme_bounds(m.synthetic_problem(1000, 64, 8, 3)),          # 32 words, compile-time form
@@ -50,12 +50,12 @@ def test_candidate_keys_and_search_match_the_restatement(ref_lib, name):
     sess.close()
 
 
-def test_share_beyond_the_list_matches_the_32bit_epilogue():
+def test_share_beyond_the_list_matches_the_popcount_schedule():
     """A round of KAO_MAX_ROUND_SIZE candidates (every CTA's share walks unsorted), with the edge bounds: same keys,
-    trajectory and base as the 32-bit epilogue."""
+    trajectory and base as the popcount schedule."""
     pb = with_extreme_bounds(m.synthetic_problem(1000, 64, 8, 3))
     a, b = session(pb), kao.Session(kao.Problem.from_fields(pb))
-    assert b.set_schedule(*WIDE)
+    assert b.set_schedule(*POPCOUNT)
     size = 1 << 24
     for rnd in (2, 3):
         assert np.array_equal(a.candidate_keys(SEED, rnd, size, 0, size), b.candidate_keys(SEED, rnd, size, 0, size)), rnd

@@ -57,12 +57,12 @@ def test_search_matches_the_restatement(ref_lib, name):
     sess.close()
 
 
-def test_share_beyond_the_list_walks_unsorted():
+def test_share_beyond_the_list_matches_the_popcount_schedule():
     """A round of KAO_MAX_ROUND_SIZE candidates: every CTA's share (127,000 candidates) is larger than any list the
-    shared memory holds.  Same keys as the schedule without sorting."""
+    shared memory holds.  Same keys as the popcount schedule, which does not sort."""
     pb = m.synthetic_problem(1000, 64, 8, 3)
     a, b = session(pb), kao.Session(kao.Problem.from_fields(pb))
-    assert b.set_schedule(1, 0x200, 512)
+    assert b.set_schedule(4, 0x22, 1024)
     size = 1 << 24
     for rnd in (2, 3):
         ka = a.candidate_keys(SEED, rnd, size, 0, size)

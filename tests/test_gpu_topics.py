@@ -211,7 +211,7 @@ def test_what_a_topic_session_does_not_offer_is_refused():
     assert refused(lib.kao_candidate_keys(h, C.c_uint64(1), C.c_uint32(0), C.c_uint32(16), C.c_uint32(0), C.c_uint32(16),
                                           C.c_void_p(keys.ctypes.data)))
     assert refused(lib.kao_set_evaluator(h, C.c_int32(0)))
-    assert refused(lib.kao_set_schedule(h, C.c_int32(1), C.c_int32(0x200), C.c_int32(512)))
+    assert refused(lib.kao_set_schedule(h, C.c_int32(1), C.c_int32(0x300), C.c_int32(512)))
     assert refused(lib.kao_round_launch(h, C.c_uint64(1), C.c_uint32(0), C.c_uint32(16), C.c_uint32(0), C.c_uint32(16),
                                         C.c_void_p(keys.ctypes.data), null))
     assert refused(lib.kao_round_apply(h, C.c_uint64(1), C.c_uint32(0), C.c_uint32(16), C.c_void_p(keys.ctypes.data), null))

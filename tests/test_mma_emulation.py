@@ -1,6 +1,7 @@
-"""The column-major evaluator with its sums on the tensor cores (csrc/kao_device_mma.cuh, schedules with pop 0x100)
-under the warp emulator (tests/emu, pop 0x100): ldmatrix and the binary MMA are restated with their PTX
-fragment layouts, and 32 candidates are generated, parked and evaluated together as one warp of the search kernel does it.
+"""The column-major evaluator with its sums on the tensor cores (csrc/kao_device_mma.cuh, schedule pop 0x300)
+under the warp emulator (tests/emu): ldmatrix and the binary MMA are restated with their PTX fragment layouts, and
+32 candidates are generated, parked and evaluated together as one warp of the search kernel does it, in index order
+(as a CTA whose share of a round exceeds its sorted list walks them).
 Keys and trajectories must be the restatement's, bit for bit."""
 import numpy as np
 import pytest
@@ -28,7 +29,7 @@ def emu():
 
 @pytest.fixture(scope="module")
 def mma(emu):
-    return lambda pb: emu.MmaSession(pb, 0x100)
+    return lambda pb: emu.MmaSession(pb, 0x300)
 
 
 def product(pb):

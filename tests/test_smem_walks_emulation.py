@@ -42,7 +42,7 @@ def emu():
 
 @pytest.fixture(scope="module")
 def mma(emu):
-    return lambda pb: emu.MmaSession(pb, 0x100)
+    return lambda pb: emu.MmaSession(pb, 0x300)
 
 
 def product(pb):

@@ -1,6 +1,6 @@
 // bmma_probe.cu — rate of the binary tensor-core MMA (mma.sync.m16n8k256 .b1 .and.popc) on this GPU.
 //
-// The column-major evaluator's MMA body (kao_device_t.cuh, kSums == 1) forms its sums with this instruction; its
+// The column-major evaluator's MMA body (kao_device_mma.cuh, schedule pop 0x300) forms its sums with this instruction; its
 // cost per candidate is the number of MMAs times the rate measured here.  Two streams per warp:
 //   dependent    every MMA accumulates onto the previous one's result: the latency of one MMA
 //   independent  kInd accumulators per warp, every warp of a full SM issuing: the throughput of an SM

@@ -73,7 +73,7 @@ def round_rows(r, rounds, kind):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--schedule", action="append", help="sync,pop(hex),threads; default: every tensor-core schedule")
+    ap.add_argument("--schedule", action="append", help="sync,pop(hex),threads; default: the default schedule")
     ap.add_argument("--rounds", type=int, default=32)
     ap.add_argument("--round-size", type=int, default=1 << 18)
     ap.add_argument("--steps", type=int, default=20, help="bench.py-style steps timed per schedule")
@@ -96,7 +96,7 @@ def main():
 
     lib = optimizer.load_library()
     scheds = [tuple(int(x, 16) if i == 1 else int(x) for i, x in enumerate(s.split(","))) for s in a.schedule] if a.schedule \
-        else [s for s in tuning.SCHEDULES if s[1] >> 8]
+        else [tuning.DEFAULT_SCHEDULE]
     print("card (name, power limit, max SM clock, SM clock): %s" % card())
     pb = kao.synthetic_problem(1000, 64, 8, 3, 0)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda:0")     # > 50 MB L2, as bench.py
