@@ -273,6 +273,28 @@ int kao_solve_fixed(const kao_problem *pb, const kao_topics *tp, const kao_repli
 int kao_objective_bound_fixed(const kao_problem *pb, const kao_replication *rp, const uint8_t *fixed,
                               const int32_t *replicas, int64_t *bound);
 
+/*
+ * Leaders only (docs/MODEL.md §13): "spread leadership, move no data".  Every partition keeps the replica set cur[p]
+ * lists; the call chooses each one's leader among those replicas, exactly.  C1, C3, C5, C6, C7 and the C3t rows of `tp`
+ * are then constants (their violation is *fixed_violation); C2 holds by construction; the free rows are C4 and the C4t
+ * rows of `tp` (tp == NULL: none).  The result is the lexicographic optimum: the least violation of the free rows, then
+ * the largest objective (README.md:145-146) among the choices with that violation.  fixed[p] = 1 (fixed == NULL: none)
+ * keeps partition p's current leader, which still counts in C4 and C4t.  Host-side, needs no GPU; the same input gives
+ * the same lists.
+ * Result: res->replicas[P*RF] = per row the chosen leader, then the row's other replicas in their order in cur, -1
+ * padded (a row whose leader stays comes back exactly as cur lists it); violation = the whole violation of that
+ * assignment as kao_eval scores it (plus the topic rows of `tp`); moves, n_candidates, rounds_run, restarts, key and
+ * device_ms = 0; objective_bound = objective, the optimum over LEADER-ONLY assignments of these replica sets, not a
+ * bound on the full program (kao_solve*'s reassignments may do better); optimal = feasible = (violation == 0);
+ * KAO_INFEASIBLE when violation > 0, with the result filled.
+ * KAO_E_ARG before anything else, naming the partition or broker: what kao_create refuses in pb; a row with an entry
+ * after a -1 (a replica on a broker outside the target list, whose data would have to move) or naming a broker not in
+ * 0..B-1; a row naming one broker twice; an empty row; a row of more than RF replicas; topic rows kao_create_topics
+ * refuses.  A trailing -1 is padding: that row is shorter, and C1 counts what it lacks.
+ */
+int kao_solve_leaders(const kao_problem *pb, const kao_topics *tp, const uint8_t *fixed, kao_result *res,
+                      int64_t *fixed_violation);
+
 int kao_destroy(kao_handle *h);
 /* base <- current assignment restricted to the target brokers and completed to RF (MODEL §4) */
 int kao_reset(kao_handle *h);

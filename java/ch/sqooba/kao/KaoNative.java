@@ -39,6 +39,21 @@ public final class KaoNative {
                                    int roundSize, int device, int nGpus, int flags, int[] replicasOut,
                                    long[] statsOut);
 
+    /**
+     * kao_solve_leaders() (docs/MODEL.md 13): every partition keeps its replicas and its leader is chosen among them,
+     * exactly; no data moves and no GPU is used.  Same tables as {@link #solve}.
+     *
+     * @param topicOf     [P] topic of each partition, or null: no per-topic leader rows (C4t)
+     * @param topicBounds [4*T] rep_lo, rep_hi, ldr_lo, ldr_hi per topic (each [T]); ignored when topicOf is null
+     * @param fixed       [P] 1 = the partition keeps its current leader, or null
+     * @param replicasOut [P*RF] leader first, then the other replicas in their current order, -1 padded
+     * @param statsOut    [3] objective, violation, the part of the violation the replica sets fix
+     * @return 0 ok, 1 every choice of leaders violates a row; throws KaoException on argument errors
+     */
+    public static native int solveLeaders(int P, int B, int R, int RF, int RFcur, byte[] rackOf, short[] wF,
+                                          short[] wL, int[] bounds, int[] cur, int[] topicOf, int[] topicBounds,
+                                          byte[] fixed, int[] replicasOut, long[] statsOut);
+
     public static final class KaoException extends RuntimeException {
         public final int code;
         public KaoException(int code, String message) { super(message); this.code = code; }

@@ -8,7 +8,7 @@ solve with a GPU candidate search behind the C ABI of ``include/kao.h`` (``libka
 There is no CPU fallback: importing works without a GPU, solving raises ``KaoError``.
 """
 from .problem import Problem, ReplicationRows, TopicRows, build_problem, default_bounds, default_weights, synthetic_problem, topic_rows  # noqa: F401
-from .optimizer import AssignmentOptimizer, KaoError, Session, SolveResult, key_obj_bits, lp_bound, objective_bound, unpack_key  # noqa: F401
+from .optimizer import AssignmentOptimizer, KaoError, Session, SolveResult, key_obj_bits, lp_bound, objective_bound, solve_leaders, unpack_key  # noqa: F401
 
 __all__ = ["Problem", "ReplicationRows", "TopicRows", "build_problem", "default_bounds", "default_weights", "synthetic_problem", "topic_rows",
-           "AssignmentOptimizer", "KaoError", "Session", "SolveResult", "key_obj_bits", "lp_bound", "objective_bound", "unpack_key"]
+           "AssignmentOptimizer", "KaoError", "Session", "SolveResult", "key_obj_bits", "lp_bound", "objective_bound", "solve_leaders", "unpack_key"]

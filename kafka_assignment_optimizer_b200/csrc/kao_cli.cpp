@@ -387,6 +387,89 @@ void emit_lp(const Model &m, std::ostream &o, bool topics)
     o << ";\n";
 }
 
+// --leaders-only (docs/MODEL.md §13): the restricted program in the same text format, leader variables on the current
+// replicas only (a fixed row: on its current leader only), C2 per partition, C4 per broker and, with topics, C4t per
+// (topic, broker).  The replica sets fix the rest, so the follower weight of every replica is a constant W0, given in a
+// first comment line: the program's optimum plus W0 is the objective.  A row whose sum has no variable gets a zero term
+// on the first variable, so that an unreachable lower bound stays in the program.
+void emit_leaders_lp(const Model &m, std::ostream &o, bool topics)
+{
+    auto var = [&](int b, int p) { return "t1b" + std::to_string(m.broker_ids[b]) + "p" + std::to_string(p) + "_l"; };
+    auto choices = [&](int p) {                             // the brokers row p may be led from
+        std::vector<int> out;
+        for (int i = 0; i < m.RFcur; ++i) {
+            const int b = m.cur[(size_t)p * m.RFcur + i];
+            if (b >= 0) out.push_back(b);
+            if (b >= 0 && m.is_fixed(p)) break;
+        }
+        return out;
+    };
+    long W0 = 0;
+    for (int p = 0; p < m.P; ++p)
+        for (int i = 0; i < m.RFcur; ++i)
+            if (m.cur[(size_t)p * m.RFcur + i] >= 0) W0 += m.wF[(size_t)p * m.B + m.cur[(size_t)p * m.RFcur + i]];
+    o << "// Leaders only: every replica stays where it is; follower weight of every replica W0 = " << W0 << "\n";
+    o << "// Optimization function, based on current assignment: leader weight less follower weight\nmax: ";
+    bool first = true;
+    for (int p = 0; p < m.P; ++p)
+        for (int b : choices(p)) {
+            const int g = (int)m.wL[(size_t)p * m.B + b] - (int)m.wF[(size_t)p * m.B + b];
+            if (g) { o << (first ? "" : " + ") << g << " " << var(b, p); first = false; }
+        }
+    const std::string any = var(m.cur[0] >= 0 ? m.cur[0] : choices(0)[0], 0);
+    auto sum_row = [&](const std::vector<std::pair<int, int>> &terms, const char *op, long rhs) {
+        for (size_t i = 0; i < terms.size(); ++i) o << (i ? " + " : "") << var(terms[i].first, terms[i].second);
+        if (terms.empty()) o << "0 " << any;
+        o << op << rhs << ";\n";
+    };
+    o << ";\n\n// Constraint on having one and only one leader per partition\n";
+    for (int p = 0; p < m.P; ++p) {
+        std::vector<std::pair<int, int>> t;
+        for (int b : choices(p)) t.emplace_back(b, p);
+        sum_row(t, " = ", 1);
+    }
+    o << "\n// Constraint on min/max leaders per broker\n";
+    for (int b = 0; b < m.B; ++b) {
+        std::vector<std::pair<int, int>> t;
+        for (int p = 0; p < m.P; ++p)
+            for (int c : choices(p)) if (c == b) t.emplace_back(b, p);
+        sum_row(t, " <= ", m.ldr_hi[b]);
+        sum_row(t, " >= ", m.ldr_lo[b]);
+    }
+    for (int tt = 0; topics && tt < (int)m.topic_names.size(); ++tt) {
+        o << "\n// Constraint on min/max leaders of topic " << m.topic_names[tt] << " per broker\n";
+        for (int b = 0; b < m.B; ++b) {
+            std::vector<std::pair<int, int>> t;
+            for (int p = 0; p < m.P; ++p)
+                if (m.topic_of[p] == tt)
+                    for (int c : choices(p)) if (c == b) t.emplace_back(b, p);
+            sum_row(t, " <= ", m.tldr_hi[tt]);
+            sum_row(t, " >= ", m.tldr_lo[tt]);
+        }
+    }
+    o << "\n// All variables are binary\nbin\n";
+    first = true;
+    for (int p = 0; p < m.P; ++p)
+        for (int b : choices(p)) { o << (first ? "" : ", ") << var(b, p); first = false; }
+    o << ";\n";
+}
+
+// --leaders-only keeps every replica: a row with a replica outside --brokers, a broker twice or no replica is refused
+void check_leader_rows(const Model &m, const std::vector<int> &brokers)
+{
+    const std::set<int> ids(brokers.begin(), brokers.end());
+    for (const Row &r : m.rows) {
+        const std::string at = "--leaders-only: partition " + r.topic + "-" + std::to_string(r.partition);
+        if (r.replicas.empty()) throw std::runtime_error(at + " has no replica");
+        for (int b : r.replicas)
+            if (!ids.count(b))
+                throw std::runtime_error(at + " has a replica on broker " + std::to_string(b) + ", which is not in --brokers: "
+                                         "its data would have to move, which takes a reassignment without --leaders-only");
+        if (std::set<int>(r.replicas.begin(), r.replicas.end()).size() != r.replicas.size())
+            throw std::runtime_error(at + " lists a broker twice");
+    }
+}
+
 std::string slurp(const std::string &path)
 {
     if (path == "-") { std::stringstream ss; ss << std::cin.rdbuf(); return ss.str(); }
@@ -405,12 +488,48 @@ std::vector<std::string> split(const std::string &s, char sep)
     return out;
 }
 
+// --leaders-only: kao_solve_leaders; the JSON lists the partitions whose leader changes, each with its other replicas in
+// their current order, for `kafka-reassign-partitions --execute` and then a preferred-leader election
+int solve_leaders(const Model &m, const kao_problem &pb, const kao_topics *tp, bool stats)
+{
+    std::vector<int32_t> reps((size_t)m.P * m.RF, -1);
+    kao_result res{};
+    res.replicas = reps.data();
+    int64_t fixed_violation = 0;
+    const int rc = kao_solve_leaders(&pb, tp, m.fixed.empty() ? nullptr : m.fixed.data(), &res, &fixed_violation);
+    if (rc < 0) { std::fprintf(stderr, "kao-cli: %s\n", kao_last_error()); return 1; }
+    if (rc == KAO_INFEASIBLE)
+        std::fprintf(stderr, "kao-cli: warning: every choice of leaders violates the constraints (violation %lld, %lld of it "
+                             "fixed by the replica sets)\n", (long long)res.violation, (long long)fixed_violation);
+    std::vector<int> changed;
+    for (int p = 0; p < m.P; ++p)
+        if (reps[(size_t)p * m.RF] != m.cur[(size_t)p * m.RFcur]) changed.push_back(p);
+    std::cout << "{\"version\":1,\"partitions\":[\n";
+    for (size_t k = 0; k < changed.size(); ++k) {
+        const int p = changed[k];
+        std::cout << "    {\"topic\":\"" << m.rows[p].topic << "\",\"partition\":" << m.rows[p].partition << ",\"replicas\":[";
+        for (int i = 0; i < m.RF && reps[(size_t)p * m.RF + i] >= 0; ++i)
+            std::cout << (i ? "," : "") << m.broker_ids[reps[(size_t)p * m.RF + i]];
+        std::cout << "]}" << (k + 1 < changed.size() ? "," : "") << "\n";
+    }
+    std::cout << "]}\n";
+    if (stats)
+        std::fprintf(stderr, "kao-cli: leaders only: objective %lld (optimal among leader-only plans), violation %lld, "
+                             "fixed_violation %lld, leaders_changed %zu, replica moves 0, %.2f ms total%s\n",
+                     (long long)res.objective, (long long)res.violation, (long long)fixed_violation, changed.size(), res.total_ms,
+                     m.fixed.empty() ? "" : (", " + std::to_string(std::count(m.fixed.begin(), m.fixed.end(), 1)) +
+                                             " partitions keep their leader").c_str());
+    return rc == KAO_INFEASIBLE ? 3 : 0;
+}
+
 int usage()
 {
     std::fprintf(stderr,
                  "usage: kao-cli --assignment FILE|- --brokers 0,1,2 --racks 0:a,1:b,2:a [--rf N]\n"
                  "               [--rounds 256] [--round-size 32768] [--restarts 1] [--seed 24301] [--device 0] [--delta] [--row-major] [--gpus N] [--spread-restarts] [--patience N] [--certificate] [--lp-certificate] [--topic-balance] [--emit-lp] [--stats]\n"
-                 "               [--keep-rf] [--topic-rf name:N,...] [--topics-to-move FILE]\n");
+                 "               [--keep-rf] [--topic-rf name:N,...] [--topics-to-move FILE]\n"
+                 "       kao-cli --leaders-only --assignment FILE|- --brokers ... --racks ... [--topic-balance] [--topics-to-move FILE]\n"
+                 "               [--emit-lp] [--stats]\n");
     return 2;
 }
 
@@ -420,7 +539,7 @@ int main(int argc, char **argv)
 {
     std::map<std::string, std::string> a;
     bool emit = false, stats = false, delta = false, rowmajor = false, spread = false, certificate = false, lp_certificate = false,
-         topic_balance = false, keep_rf = false;
+         topic_balance = false, keep_rf = false, leaders_only = false, column_major = false;
     for (int i = 1; i < argc; ++i) {
         std::string k = argv[i];
         if (k == "--emit-lp") { emit = true; continue; }
@@ -432,11 +551,25 @@ int main(int argc, char **argv)
         if (k == "--lp-certificate") { lp_certificate = true; continue; }  // Lagrangian LP bound (GPU): proves what the flow bound cannot
         if (k == "--topic-balance") { topic_balance = true; continue; }   // every topic spread over the brokers too
         if (k == "--keep-rf") { keep_rf = true; continue; }   // every topic keeps its own RF (docs/MODEL.md §11)
-        if (k == "--column-major") continue;                  // accepted for old scripts: it is the default now
+        if (k == "--column-major") { column_major = true; continue; }   // accepted for old scripts: it is the default now
+        if (k == "--leaders-only") { leaders_only = true; continue; }   // reorder replica lists only (docs/MODEL.md §13)
         if (k.rfind("--", 0) != 0 || i + 1 >= argc) return usage();
         a[k.substr(2)] = argv[++i];
     }
     if (!a.count("assignment") || !a.count("brokers") || !a.count("racks")) return usage();
+    if (leaders_only) {                                       // a leader-only plan moves no data and runs no search
+        const std::vector<std::pair<bool, const char *>> refused = {
+            {a.count("rf") > 0, "--rf"}, {keep_rf, "--keep-rf"}, {a.count("topic-rf") > 0, "--topic-rf"}, {delta, "--delta"},
+            {rowmajor, "--row-major"}, {column_major, "--column-major"}, {a.count("gpus") > 0, "--gpus"},
+            {a.count("restarts") > 0, "--restarts"}, {lp_certificate, "--lp-certificate"}, {certificate, "--certificate"}};
+        for (const auto &r : refused)
+            if (r.first) {
+                std::fprintf(stderr, "kao-cli: --leaders-only cannot be combined with %s: a leader-only plan keeps every "
+                                     "replica where it is and is exact, so it takes no replication factor, evaluator, GPU, "
+                                     "restart or certificate option\n", r.second);
+                return 2;
+            }
+    }
     try {
         const std::string text = slurp(a["assignment"]);
         Parser ps(text);
@@ -470,15 +603,17 @@ int main(int argc, char **argv)
         Model m = keep_rf || !topic_rf.empty()
                       ? build_model_rf(rows, brokers, racks, keep_rf, a.count("rf") ? rf : 0, topic_rf)
                       : build_model(rows, brokers, racks, rf);
+        if (leaders_only) check_leader_rows(m, brokers);
         if (a.count("topics-to-move")) {                      // Kafka's {"topics":[{"topic":...}],"version":1}
             const std::string move_text = slurp(a["topics-to-move"]);
             Parser pt(move_text);
             const Json tdoc = pt.value();
             std::set<std::string> move;
             for (const Json &e : tdoc.at("topics").arr) move.insert(e.at("topic").str);
-            fix_rows(m, move, brokers, topic_rf, topic_balance && !emit);   // --emit-lp shifts each (topic, broker) row
+            // --emit-lp shifts each (topic, broker) row; leader-only plans take a fixed row in any topic
+            fix_rows(m, move, brokers, topic_rf, topic_balance && !emit && !leaders_only);
         }
-        if (emit) { emit_lp(m, std::cout, topic_balance); return 0; }
+        if (emit) { (leaders_only ? emit_leaders_lp : emit_lp)(m, std::cout, topic_balance); return 0; }
 
         kao_problem pb{};
         pb.P = m.P; pb.B = m.B; pb.R = m.R; pb.RF = m.RF; pb.RFcur = m.RFcur;
@@ -486,6 +621,9 @@ int main(int argc, char **argv)
         pb.rep_lo = m.rep_lo.data(); pb.rep_hi = m.rep_hi.data(); pb.ldr_lo = m.ldr_lo.data(); pb.ldr_hi = m.ldr_hi.data();
         pb.rack_lo = m.rack_lo.data(); pb.rack_hi = m.rack_hi.data(); pb.ppr_lo = m.ppr_lo; pb.ppr_hi = m.ppr_hi;
         pb.cur = m.cur.data();
+        kao_topics tp{(int32_t)m.topic_names.size(), m.topic_of.data(), m.trep_lo.data(), m.trep_hi.data(),
+                      m.tldr_lo.data(), m.tldr_hi.data()};
+        if (leaders_only) return solve_leaders(m, pb, topic_balance ? &tp : nullptr, stats);
         kao_options opt{};
         opt.seed = a.count("seed") ? std::strtoull(a["seed"].c_str(), nullptr, 0) : 0x5EED;
         opt.rounds = a.count("rounds") ? (uint32_t)std::atoi(a["rounds"].c_str()) : 256;
@@ -502,8 +640,6 @@ int main(int argc, char **argv)
         std::vector<int32_t> reps((size_t)m.P * m.RF, -1);
         kao_result res{};
         res.replicas = reps.data();
-        kao_topics tp{(int32_t)m.topic_names.size(), m.topic_of.data(), m.trep_lo.data(), m.trep_hi.data(),
-                      m.tldr_lo.data(), m.tldr_hi.data()};
         kao_replication rp{m.prf.data(), m.pprlo.data(), m.pprhi.data()};
         const int rc = !m.fixed.empty() ? kao_solve_fixed(&pb, topic_balance ? &tp : nullptr, m.prf.empty() ? nullptr : &rp,
                                                           m.fixed.data(), &opt, &res)

@@ -8,6 +8,7 @@
 #include "kao_bound.hpp"
 #include "kao_lagrange.hpp"
 #include "kao_large.hpp"
+#include "kao_leaders.hpp"
 #include "../../include/kao.h"
 
 #include <chrono>
@@ -1429,6 +1430,37 @@ extern "C" int kao_objective_bound_replication(const kao_problem *pb, const kao_
         if (!build_host_model(*pb, m, why) || (rp && !build_host_replication(*rp, m, why))) return fail(KAO_E_ARG, why);
         *bound = objective_upper_bound(m, *pb);
         if (replicas) *bound = objective_flow_bound(m, *pb, replicas, *bound);
+        return KAO_OK;
+    });
+}
+// leader-only rebalancing (docs/MODEL.md §13): host-side, exact, no GPU; the replica sets stay as cur lists them
+extern "C" int kao_solve_leaders(const kao_problem *pb, const kao_topics *tp, const uint8_t *fixed, kao_result *res,
+                                 int64_t *fixed_violation)
+{
+    return guarded([&] {
+        if (!pb || !res || !res->replicas) return fail(KAO_E_ARG, "null argument");
+        const auto t0 = std::chrono::steady_clock::now();
+        LeaderPlan plan;
+        std::string why;
+        if (!solve_leaders(*pb, tp, fixed, plan, why)) return fail(KAO_E_ARG, why);
+        std::memcpy(res->replicas, plan.replicas.data(), plan.replicas.size() * sizeof(int32_t));
+        res->objective = res->objective_bound = plan.objective;
+        res->violation = plan.violation;
+        res->feasible = plan.violation == 0;
+        res->optimal = res->feasible;
+        res->moves = 0;
+        res->key = 0;
+        res->n_candidates = 0;
+        res->rounds_run = 0;
+        res->restarts = 0;
+        res->device_ms = 0;
+        res->key_obj_bits = kao_key_obj_bits(pb);
+        res->n_gpus = 0;
+        if (fixed_violation) *fixed_violation = plan.fixed_violation;
+        res->total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        if (!res->feasible) return fail(KAO_INFEASIBLE, "leaders only: the best choice of leaders still violates the rows by " +
+                                                        std::to_string(plan.violation) + " (" + std::to_string(plan.fixed_violation) +
+                                                        " of it in the rows the replica sets fix)");
         return KAO_OK;
     });
 }

@@ -64,6 +64,7 @@ def load_library():
         lib = C.CDLL(_LIB_PATH)
         lib.kao_last_error.restype = C.c_char_p
         lib.kao_version.restype = C.c_int
+        lib.kao_solve_leaders.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -213,6 +214,7 @@ class SolveResult:
     optimal: bool = False     # proven optimal: feasible and objective == objective_bound
     key_obj_bits: int = 24    # cost-field width of `key` (unpack_key)
     n_gpus: int = 1
+    fixed_violation: int = 0  # solve_leaders: the part of `violation` the replica sets fix (C1, C3, C5, C6, C7, C3t)
 
 
 class Session:
@@ -434,6 +436,31 @@ def solve(pb: Problem, seed: int = 0x5EED, rounds: int = 256, round_size: int = 
     return SolveResult(reps, res.objective, res.violation, res.moves, rc == KAO_OK, res.key,
                        res.n_candidates, res.rounds_run, res.device_ms, res.total_ms, res.objective_bound,
                        bool(res.optimal), res.key_obj_bits, res.n_gpus)
+
+
+def solve_leaders(pb: Problem, topic_balance: bool = False, topics: Optional[TopicRows] = None) -> SolveResult:
+    """Leaders only (kao_solve_leaders, docs/MODEL.md §13; host-side, needs no GPU): every partition keeps its replicas
+    and the leader is chosen among them, exactly — the least violation of C4 (and, with topic_balance, of the C4t rows
+    of `topics`, by default topic_rows(pb)), then the largest objective.  Rows come back leader first, the other replicas
+    in their order in pb.cur; pb.fixed keeps those partitions' leaders.  moves is 0, objective_bound the optimum over
+    leader-only assignments (not a bound on the full program), and fixed_violation the part of the violation the
+    replica sets fix.  Per-partition replication rows (pb.replication) ask for data movement and are refused."""
+    if pb.replication is not None:
+        raise ValueError("solve_leaders: per-partition replication factors change replica sets; leaders only keeps them "
+                         "as they are")
+    if topic_balance and topics is None:
+        topics = topic_rows(pb)
+    reps = np.full((pb.P, pb.RF), -1, np.int32)
+    res = _KaoResult()
+    res.replicas = reps.ctypes.data
+    fv = C.c_int64()
+    cp, ct = _CProblem(pb), _CTopics(topics)
+    fx = None if pb.fixed is None else _fixed(pb)
+    rc = _check(load_library().kao_solve_leaders(cp.ref(), ct.ref(), None if fx is None else C.c_void_p(fx.ctypes.data),
+                                                 C.byref(res), C.byref(fv)), allow_infeasible=True)
+    return SolveResult(reps, res.objective, res.violation, res.moves, rc == KAO_OK, res.key, res.n_candidates,
+                       res.rounds_run, res.device_ms, res.total_ms, res.objective_bound, bool(res.optimal),
+                       res.key_obj_bits, res.n_gpus, fv.value)
 
 
 def evaluate(pb: Problem, replicas, device: int = 0):

@@ -9,10 +9,10 @@ The reference only names its hosted endpoint (`/root/reference/README.md:187-194
                    "rf": 2, "rounds": 256, "round_size": 32768, "restarts": 1, "patience": 0, "delta": false,
                    "gpus": 1, "spread_restarts": false, "certificate": false,
                    "lp_certificate": false, "topic_balance": false, "keep_rf": false, "topic_rf": {},
-                   "topics_to_move": ["name", ...]}
+                   "topics_to_move": ["name", ...], "leaders_only": false}
     200           {"reassignment": {"version":1,"partitions":[...]},    README.md:67-78
                    "objective": ..., "violation": ..., "moves": ..., "feasible": ...,
-                   "objective_bound": ..., "proven_optimal": ...}
+                   "objective_bound": ..., "proven_optimal": ...}     (+ "fixed_violation" with leaders_only)
 
 `gpus` > 1 shards every round over that many GPUs (or, with `spread_restarts`, runs the restarts side by side);
 `certificate` asks for the flow bound, so that `proven_optimal` can say the answer is what lp_solve would return
@@ -23,13 +23,19 @@ replication factor (the length of its longest replica list) and `topic_rf` ({"to
 topics, the others keeping theirs or taking `rf` when it is given (per-partition rows, docs/MODEL.md §11).
 `topics_to_move` searches only those topics and the partitions that must leave a broker, keeps every other partition
 where it is (still counted in every balance row, docs/MODEL.md §12) and returns only the searched partitions, as
-`kafka-reassign-partitions --generate` does for its topics-to-move.json.
+`kafka-reassign-partitions --generate` does for its topics-to-move.json.  `leaders_only` moves no data: it chooses every
+partition's leader among its current replicas, exactly (`solve_leaders`, docs/MODEL.md §13; no GPU, no search), and
+returns the partitions whose leader changes, for `--execute` and a preferred-leader election.  It takes `topic_balance`
+and `topics_to_move` (those partitions keep their leader) and refuses `keep_rf`, `topic_rf`, an `rf` other than the
+rows' length and a replica on a broker outside `brokers`; `fixed_violation` is the part of the violation the replica
+sets fix.
 
 `python -m kafka_assignment_optimizer_b200.service --port 8080` (needs a GPU: there is no CPU path).
 """
 from __future__ import annotations
 
 import argparse
+import dataclasses
 import json
 from http.server import BaseHTTPRequestHandler, ThreadingHTTPServer
 from typing import Callable, Optional
@@ -58,6 +64,8 @@ def handle_submit(body: dict, solver: Optional[Callable] = None) -> dict:
     racks = body["racks"]
     racks = parse_rack_map(racks) if isinstance(racks, str) else {int(k): str(v) for k, v in racks.items()}
     keep_rf, topic_rf = bool(body.get("keep_rf", False)), body.get("topic_rf") or None
+    if body.get("leaders_only"):
+        return _leaders_only(body, rows, topics, brokers, racks, keep_rf, topic_rf)
     # fixed rows (docs/MODEL.md §12), only when the request lists topics to move
     move = {"topics_to_move": parse_topics_to_move(body["topics_to_move"])} if "topics_to_move" in body else {}
     if keep_rf or topic_rf:
@@ -87,6 +95,30 @@ def handle_submit(body: dict, solver: Optional[Callable] = None) -> dict:
     return {"reassignment": reassignment_json(pb, res.replicas), "objective": int(res.objective),
             "violation": int(res.violation), "moves": int(res.moves), "feasible": bool(res.feasible),
             "objective_bound": int(res.objective_bound), "proven_optimal": bool(res.optimal)}
+
+
+def _leaders_only(body: dict, rows, topics, brokers, racks, keep_rf, topic_rf) -> dict:
+    from .optimizer import solve_leaders
+
+    rf = max(len(r) for r in rows)
+    if keep_rf or topic_rf or (body.get("rf") and int(body["rf"]) != rf):
+        raise ValueError("leaders_only keeps every replica where it is: it cannot be combined with keep_rf, topic_rf or an "
+                         "rf other than the rows' (%d)" % rf)
+    ids = set(brokers)
+    for (t, q), reps in zip(topics, rows):
+        out = [b for b in reps if b not in ids]
+        if out or not reps or len(set(reps)) != len(reps):
+            raise ValueError("leaders_only: partition %s-%d %s" % (t, q, "has a replica on broker %d, which is not in "
+                             "brokers: its data would have to move" % out[0] if out else "has no replica" if not reps
+                             else "lists a broker twice"))
+    move = {"topics_to_move": parse_topics_to_move(body["topics_to_move"])} if "topics_to_move" in body else {}
+    pb = build_problem(rows, brokers, racks, rf, topics, **move)
+    res = solve_leaders(pb, topic_balance=bool(body.get("topic_balance", False)))
+    changed = res.replicas[:, 0] != pb.cur[:, 0]
+    return {"reassignment": reassignment_json(dataclasses.replace(pb, fixed=~changed), res.replicas),
+            "objective": int(res.objective), "violation": int(res.violation), "moves": int(res.moves),
+            "feasible": bool(res.feasible), "objective_bound": int(res.objective_bound), "proven_optimal": bool(res.optimal),
+            "fixed_violation": int(res.fixed_violation)}
 
 
 class _Handler(BaseHTTPRequestHandler):
