@@ -55,7 +55,7 @@ struct Params {
     const uint32_t *swT;         // packed weight entries [4][Ppad]: slot | wF << 8 | wL << 20
     const uint32_t *planesT;     // weighted mask planes [nplanes][W][Ppad], or nullptr
     const uint32_t *dense_w;     // [P][NS] wF | wL << 16, or nullptr
-    const uint32_t *homeT;       // [Ppad] 4 x u8 home slots (0xFF = none)
+    const uint32_t *homeT;       // [Ppad] 4 x u8 home slots, then [Ppad] u8 validity nibbles (home_ok below)
     // term planes of the sparse objective (column-major evaluator, kao_device_t.cuh; host: kao_host.hpp)
     int nz;                      // planes in use (0..8)
     int z_on_leader;             // bit j set: plane j counts leaderships (bonus wL - wF), else replicas (wF)
@@ -71,6 +71,29 @@ struct Params {
 inline void set_rf_masks(Params &p)
 {
     for (int k = 0; k < 4; ++k) p.rf_mask[k] = ((p.RF >> k) & 1) ? 0xFFFFFFFFu : 0u;
+}
+
+// Home slots (docs/MODEL.md §5.1): byte i of homeT[p] is the slot of cur[p][i] (i < 4), and an entry without a
+// surviving broker is "none".  Rows of at most 128 slots (W <= 4) never use slot 255, so there the byte 0xFF says
+// "none".  In eight-word rows slot 255 is a broker when B = 256, so the Ppad bytes after the Ppad words hold one
+// validity nibble per partition (bit i: byte i is a home slot), and only W = 8 code reads them.
+template <int W> __host__ __device__ __forceinline__ uint32_t home_valid(const uint32_t *homeT, int Ppad, int p)
+{
+    if constexpr (W == 8) return reinterpret_cast<const uint8_t *>(homeT + Ppad)[p];
+    else return 0u;
+}
+// byte i of a home word, hs, is a home slot; hv = home_valid<W>(...) of the same partition
+template <int W> __host__ __device__ __forceinline__ bool home_ok(int hs, uint32_t hv, int i)
+{
+    if constexpr (W == 8) return (hv >> i) & 1u;
+    else return hs != 0xFF;
+}
+// home0: the slot of cur[p][0], -1 if that broker does not survive
+template <int W> __host__ __device__ __forceinline__ int home0(const uint32_t *homeT, int Ppad, int p)
+{
+    const int h0 = homeT[p] & 0xFF;
+    if constexpr (W == 8) return (home_valid<W>(homeT, Ppad, p) & 1u) ? h0 : -1;
+    else return (h0 == 0xFF) ? -1 : h0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -426,7 +449,7 @@ template <int W, bool kThread = false, bool kSmall = false, bool kMerged = false
             read_row(p, row, ld);
             lo = (int)ld;
             int want = -1;
-            if (guided) { const int h0 = d->homeT[p] & 0xFF; want = (h0 == 0xFF) ? -1 : h0; }
+            if (guided) want = home0<W>(d->homeT, d->Ppad, p);
             hi = pick_leader(row, ld, want, r[2]);
             if (hi < 0) return;
             push(ps, p, row, ld, rows);
@@ -439,14 +462,14 @@ template <int W, bool kThread = false, bool kSmall = false, bool kMerged = false
             int a = row_kth<W, kSmall>(row, (int)mulhi32(r[2], (uint32_t)n));
             int o = (int)mulhi32(r[3], (uint32_t)B);
             if (guided) {
-                const uint32_t h4 = d->homeT[p];
+                const uint32_t h4 = d->homeT[p], hv = home_valid<W>(d->homeT, d->Ppad, p);
                 uint32_t home[W], miss[W], nonhome[W];
 #pragma unroll
                 for (int t = 0; t < W; ++t) home[t] = 0;
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int hs = (h4 >> (8 * i)) & 0xFF;
-                    if (hs != 0xFF && !row_has<W>(home, hs)) row_flip<W>(home, hs);
+                    if (home_ok<W>(hs, hv, i) && !row_has<W>(home, hs)) row_flip<W>(home, hs);
                 }
 #pragma unroll
                 for (int t = 0; t < W; ++t) { miss[t] = home[t] & ~row[t]; nonhome[t] = row[t] & ~home[t]; }
@@ -517,7 +540,7 @@ template <int W, bool kThread = false, bool kSmall = false, bool kMerged = false
                     if (link == 0) hi = moved_to; else lo = a;
                 } else {                                       // L-push / L-pull: one LEADER step
                     int want = lo;
-                    if (link == 2 && !close) { const int h0 = d->homeT[q] & 0xFF; want = (h0 == 0xFF) ? -1 : h0; }
+                    if (link == 2 && !close) want = home0<W>(d->homeT, d->Ppad, q);
                     const int old = (int)lq;
                     const int t = pick_leader(rq, lq, want, rb);
                     if (t < 0) return;
@@ -575,7 +598,7 @@ template <int W, bool kThread = false, bool kSmall = false, bool kMerged = false
                 if (q < 0) return;
                 read_row(q, rq, lq);
                 int want = lo;
-                if (!close) { const int h0 = d->homeT[q] & 0xFF; want = (h0 == 0xFF) ? -1 : h0; }
+                if (!close) want = home0<W>(d->homeT, d->Ppad, q);
                 const int t = pick_leader(rq, lq, want, rb);
                 if (t < 0) return;
                 hi = t;

@@ -78,7 +78,7 @@ apply_winner_kernel(Params d, uint64_t seed, uint32_t round, uint32_t round_size
     }
     __threadfence_block();
     __syncthreads();
-    rebuild_lists<1024>(d.bitsT, d.leader, d.homeT, d.P, d.Ppad, d.D, d.DL, d.nD, s_scan);
+    rebuild_lists<W, 1024>(d.bitsT, d.leader, d.homeT, d.P, d.Ppad, d.D, d.DL, d.nD, s_scan);
 }
 
 __global__ void fill_u64_kernel(unsigned long long *p, unsigned long long v, size_t n)
@@ -499,7 +499,7 @@ static int create_impl(const kao_problem *pb, const kao_topics *tp, const kao_re
     CUDA_TRY(dalloc(h, &h->d_bits, (size_t)W * Ppad * 4));
     CUDA_TRY(dalloc(h, &h->d_leader, (size_t)Ppad));
     CUDA_TRY(dalloc(h, &h->d_sw, (size_t)4 * Ppad * 4));
-    CUDA_TRY(dalloc(h, &h->d_home, (size_t)Ppad * 4));
+    CUDA_TRY(dalloc(h, &h->d_home, m.homeT.size() * 4));
     // the large path keeps two buffers per displaced list (kao_large.hpp), its transposed planes and winner record
     const size_t nlists = h->large ? 2 : 1;
     CUDA_TRY(dalloc(h, &h->d_D, nlists * Ppad * 2));

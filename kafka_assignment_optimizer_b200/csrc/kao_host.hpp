@@ -44,7 +44,7 @@ struct HostModel {
     struct Cell { int p, b; uint32_t f, l; }; // a non-zero cell of the weight tables: follower / leader weight of (p, broker)
     std::vector<Cell> cells;                  // all of them, by partition then broker
     std::vector<int> cell_first;              // [P + 1] cells of partition p: cell_first[p] .. cell_first[p + 1]
-    std::vector<uint32_t> homeT;              // [Ppad]
+    std::vector<uint32_t> homeT;              // [Ppad] home slots, then [Ppad] u8 validity nibbles
     // per-partition C1 / C7 rows (kao_replication, docs/MODEL.md §11); empty: RF and ppr_lo .. ppr_hi for every row
     std::vector<uint8_t> rf_p, ppr_lo_p, ppr_hi_p;
     int rf(int p) const { return rf_p.empty() ? RF : rf_p[p]; }
@@ -269,13 +269,19 @@ inline bool build_host_model(const kao_problem &pb, HostModel &m, std::string &w
         }
     }
     m.hi1 = (pb.ppr_lo == 0 && pb.ppr_hi == 1);
-    // home slots: the first four surviving entries of cur[p]
-    m.homeT.assign((size_t)m.Ppad, 0xFFFFFFFFu);
+    // home slots: the slots of the surviving entries among the first four positions of cur[p], byte i for cur[p][i]
+    // (0xFF: none), then one validity nibble per partition (kao_device.cuh, home_valid: 0xFF is slot 255 when B = 256)
+    m.homeT.assign((size_t)m.Ppad + m.Ppad / 4, 0xFFFFFFFFu);
+    uint8_t *valid = reinterpret_cast<uint8_t *>(m.homeT.data() + m.Ppad);
+    std::fill(valid, valid + m.Ppad, 0);
     for (int p = 0; p < pb.P; ++p) {
         uint32_t h = 0xFFFFFFFFu;
         for (int i = 0; i < pb.RFcur && i < 4; ++i) {
             const int b = m.cur[(size_t)p * pb.RFcur + i];
-            if (b >= 0) h = (h & ~(0xFFu << (8 * i))) | ((uint32_t)m.slot_of_broker[b] << (8 * i));
+            if (b >= 0) {
+                h = (h & ~(0xFFu << (8 * i))) | ((uint32_t)m.slot_of_broker[b] << (8 * i));
+                valid[p] |= (uint8_t)(1u << i);
+            }
         }
         m.homeT[p] = h;
     }

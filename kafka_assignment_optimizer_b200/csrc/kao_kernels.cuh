@@ -241,7 +241,7 @@ search_round_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t round, uint
 
 // Rebuilds the displaced lists of a base with the whole block (ballot compaction, ascending
 // order).  cnt: 2 x 36 ints of shared scratch.  counts[0] = |D|, counts[1] = |DL|.
-template <int THREADS>
+template <int W, int THREADS>
 __device__ __forceinline__ void rebuild_lists(const uint32_t *bitsT, const uint8_t *leader, const uint32_t *homeT,
                                               int P, int Ppad, uint16_t *D, uint16_t *DL, int *counts, int *cnt)
 {
@@ -253,11 +253,11 @@ __device__ __forceinline__ void rebuild_lists(const uint32_t *bitsT, const uint8
         const int p = p0 + tid;
         bool miss = false, ldis = false;
         if (p < P) {
-            const uint32_t h4 = homeT[p];
+            const uint32_t h4 = homeT[p], hv = home_valid<W>(homeT, Ppad, p);
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int hs = (h4 >> (8 * i)) & 0xFF;
-                if (hs != 0xFF) {
+                if (home_ok<W>(hs, hv, i)) {
                     const bool has = (bitsT[(size_t)(hs >> 5) * Ppad + p] >> (hs & 31)) & 1u;
                     miss |= !has;
                     if (i == 0) ldis = has && ((int)leader[p] != hs);
@@ -528,7 +528,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
     mbar_wait(s_bar, 0);
     if constexpr (has_oh_plane<Cfg>()) build_oh_plane<W, THREADS>(s_bits, s_leader, d.Ppad);
     if constexpr (Cfg::kTrans) build_t_planes<W, THREADS, cfg_mma<Cfg>()>(d, s_sw, s_z, s_bits, s_leader);
-    rebuild_lists<THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
+    rebuild_lists<W, THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
     if constexpr (Cfg::kTrans) {
         // s_counts[2] = partitions whose leader slot is not one of their replicas (0 for every base the engine builds or
         // reaches itself): while it is 0 the leader plane T1 also answers the generator's "is led from slot s"
@@ -917,7 +917,7 @@ search_persistent_kernel(Params d, SmemPlan plan, uint64_t seed, uint32_t first_
         }
         __syncthreads();
         KAO_PHASE(if (ph) ph[kPhApply] = clock64();)
-        rebuild_lists<THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
+        rebuild_lists<W, THREADS>(s_bits, s_leader, d.homeT, d.P, d.Ppad, s_D, s_DL, s_counts, s_scan);
         KAO_PHASE(if (ph) ph[kPhRebuild] = clock64();)
 #if !defined(KAO_NO_PATIENCE)
         if (s_red[kWarps]) break;

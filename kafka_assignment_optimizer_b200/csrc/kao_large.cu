@@ -95,13 +95,14 @@ __device__ __forceinline__ Gen<W, true, true> large_gen(const Params &d, const L
 // membership of partition p (row, leader) in the displaced lists (as rebuild_lists decides it): a home slot is
 // missing (D); the first home slot is held but does not lead (DL)
 template <int W>
-__device__ __forceinline__ void displaced(uint32_t h4, const uint32_t (&row)[W], uint32_t ld, bool &miss, bool &ldis)
+__device__ __forceinline__ void displaced(uint32_t h4, uint32_t hv, const uint32_t (&row)[W], uint32_t ld, bool &miss,
+                                          bool &ldis)
 {
     miss = false; ldis = false;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int hs = (h4 >> (8 * i)) & 0xFF;
-        if (hs != 0xFF) {
+        if (home_ok<W>(hs, hv, i)) {
             const bool has = row_has<W>(row, hs);
             miss |= !has;
             if (i == 0) ldis = has && ((int)ld != hs);
@@ -156,9 +157,9 @@ __device__ void apply_winner_large(const Params &d, const LargeArgs &la, const C
                 const bool was = (int)lo < NSL && row_has<W>(xo, (int)lo), is = (int)ln < NSL && row_has<W>(xn, (int)ln);
                 nbad += (was ? 0 : -1) + (is ? 0 : 1);
                 bool mo, lo_dis, mn, ln_dis;
-                const uint32_t h4 = d.homeT[p];
-                displaced<W>(h4, xo, lo, mo, lo_dis);
-                displaced<W>(h4, xn, ln, mn, ln_dis);
+                const uint32_t h4 = d.homeT[p], hv = home_valid<W>(d.homeT, d.Ppad, p);
+                displaced<W>(h4, hv, xo, lo, mo, lo_dis);
+                displaced<W>(h4, hv, xn, ln, mn, ln_dis);
                 if (mo && !mn) lc.del[0][lc.nd[0]++] = p;
                 if (!mo && mn) lc.ins[0][lc.ni[0]++] = p;
                 if (lo_dis && !ln_dis) lc.del[1][lc.nd[1]++] = p;
@@ -453,7 +454,7 @@ __global__ void __launch_bounds__(1024, 1) large_lists_kernel(Params d)
 {
     __shared__ int s_scan[72];
     __shared__ int s_bad;
-    rebuild_lists<1024>(d.bitsT, d.leader, d.homeT, d.P, d.Ppad, d.D, d.DL, d.nD, s_scan);
+    rebuild_lists<W, 1024>(d.bitsT, d.leader, d.homeT, d.P, d.Ppad, d.D, d.DL, d.nD, s_scan);
     if (threadIdx.x == 0) s_bad = 0;
     __syncthreads();
     int bad = 0;

@@ -273,7 +273,7 @@ void kao_ref_init_base(const ref_problem *pb, uint32_t *bits, uint8_t *leader)
 }
 
 /* ---------------------------------------------------------------- base analysis (docs/MODEL.md §5.1) */
-/* home[p] = slots of the first KAO_HOME surviving entries of cur[p]; home0[p] = slot of cur[p][0]
+/* home[p] = slots of the surviving entries among the first KAO_HOME positions of cur[p]; home0[p] = slot of cur[p][0]
  * if that broker survives, else -1.  D = ascending list of the partitions whose row lacks at
  * least one home slot ("displaced"); DL = ascending list of the partitions that hold a replica on
  * home0 but are led from elsewhere ("leader displaced"). */

@@ -106,10 +106,11 @@ void rebuild_lists(Emu &e)
     e.nD = e.nL = 0;
     for (int p = 0; p < m.P; ++p) {
         const uint32_t h4 = m.homeT[p];
+        const uint32_t hv = m.W == 8 ? home_valid<8>(m.homeT.data(), m.Ppad, p) : 0u;
         bool miss = false, ldis = false;
         for (int i = 0; i < 4; ++i) {
             const int hs = (h4 >> (8 * i)) & 0xFF;
-            if (hs == 0xFF) continue;
+            if (!(m.W == 8 ? home_ok<8>(hs, hv, i) : home_ok<4>(hs, hv, i))) continue;
             const bool has = (e.bits[(size_t)(hs >> 5) * m.Ppad + p] >> (hs & 31)) & 1u;
             miss |= !has;
             if (i == 0) ldis = has && ((int)e.leader[p] != hs);

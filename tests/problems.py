@@ -311,11 +311,21 @@ def moved_base(pb, reps, seed):
 
 
 # ---- every one of the 256 slots a broker (docs/MODEL.md §2) -------------------------------------------------------
+def slots(pb):
+    """docs/MODEL.md §2: rack-major slots, S = pow2 >= max(8, largest rack) -> slot of every broker"""
+    size = np.bincount(pb.rack_of, minlength=pb.R)
+    S = 8
+    while S < size.max():
+        S <<= 1
+    rank = np.array([int((pb.rack_of[:b] == pb.rack_of[b]).sum()) for b in range(pb.B)])
+    return pb.rack_of.astype(int) * S + rank
+
+
 # A cluster of 255 brokers grown by one: the current assignment uses brokers 0..254, the target list is 0..255 and
 # broker b sits in rack b // (256 / racks), so broker 255 is the last of the last rack, on slot 255, with no home
-# replica there (a home replica on slot 255 is DESIGN.md 7.1's known limit).  Slot 255 is then a real broker while
-# several tables use the byte 0xFF for "none" or "padding"; the new broker is empty, so every balance row that binds
-# on it (C3 / C4, and the topic rows of the labellings below) reads its slot.
+# replica there (HOME255_SHAPES below put home replicas there).  Slot 255 is then a real broker while several tables
+# use the byte 0xFF for "none" or "padding"; the new broker is empty, so every balance row that binds on it (C3 / C4,
+# and the topic rows of the labellings below) reads its slot.
 def grown_by_one(P, racks, RF=3, seed=0):
     rng = np.random.RandomState(seed)
     per = 256 // racks
@@ -377,5 +387,90 @@ def leader_on_255_removed():
     return m.build_problem(cur, list(range(256)), {b: "r%02d" % (min(b, 255) // 16) for b in range(260)}, 3)
 
 
-# initial-base checks only: their current leaders sit on slot 255 (a home slot there, DESIGN.md 7.1), so no walks
+# initial-base checks: their current leaders sit on slot 255 and their rows get completed
 LEADER255_SHAPES = {"leader255_rf_up": leader_on_255_rf_up, "leader255_removed": leader_on_255_removed}
+
+
+# ---- home replicas on slot 255 (docs/MODEL.md §5.1) -------------------------------------------------------------------
+# 256-broker clusters as they are met: broker 255 sits on slot 255 and holds current replicas, so it is a home slot of
+# the partitions that have them.  When every slot is a broker the home byte 0xFF is slot 255 itself: the guided
+# operations and the displaced lists must count it as the restatement does.
+def full_cluster(P, racks, RF=3, seed=0):
+    """A random current assignment over all 256 brokers; broker b in rack b // (256 / racks), so broker 255 is the last
+    of the last rack, on slot 255"""
+    rng = np.random.RandomState(seed)
+    per = 256 // racks
+    current = [list(map(int, rng.choice(256, size=RF, replace=False))) for _ in range(P)]
+    return m.build_problem(current, list(range(256)), {b: "rack%02d" % (b // per) for b in range(256)}, RF)
+
+
+def rf_down_onto_255(P, seed=0):
+    """RF lowered from 4 to 3 in 16 racks of 16: every fifth partition has broker 255 fourth of four current replicas,
+    the others three replicas on other brokers.  MODEL §4 drops the fourth, so the initial base's D is exactly the
+    partitions whose one missing home is slot 255."""
+    rng = np.random.RandomState(seed)
+    current = []
+    for p in range(P):
+        row = list(map(int, rng.choice(255, size=3, replace=False)))
+        current.append(row + [255] if p % 5 == 0 else row)
+    return m.build_problem(current, list(range(256)), {b: "r%02d" % (b // 16) for b in range(256)}, 3)
+
+
+HOME255_SHAPES = {
+    "h255_r16_rr": lambda: m.synthetic_problem(1024, 256, 16, 3),      # config 5's layout: 16 racks of 16, round robin
+    "h255_r32": lambda: full_cluster(600, 32, seed=110),               # 32 racks of 8
+    "h255_r1": lambda: full_cluster(500, 1, seed=111),                 # one rack of 256: S = 256
+    "h255_rf_down": lambda: rf_down_onto_255(600, seed=103),           # RF 4 -> 3, broker 255 fourth
+    "h255_big": lambda: m.synthetic_problem(8200, 256, 16, 3, perturb=0.02, seed=5),    # the HBM path
+}
+
+
+def home_lists(pb, reps):
+    """docs/MODEL.md §5.1 written out over replica lists (leader first, -1 padded): home[p] = the surviving brokers
+    among the first four positions of cur[p]; home0[p] = cur[p][0] if it survives.  -> (D: partitions whose row lacks
+    a home broker, DL: partitions that hold home0 but are led from another broker), both ascending"""
+    D, DL = [], []
+    for p in range(pb.P):
+        row = [int(b) for b in reps[p] if b >= 0]
+        home = {int(b) for b in pb.cur[p][:4] if 0 <= b < pb.B}
+        if home - set(row):
+            D.append(p)
+        h0 = int(pb.cur[p][0])
+        if 0 <= h0 < pb.B and h0 in row and row[0] != h0:
+            DL.append(p)
+    return D, DL
+
+
+def home255_bases(pb, reps):
+    """Bases that leave the guided operations no choice but slot 255, from a base `reps` with no displaced partition
+    other than those missing only the broker on slot 255:
+    - "d255": D is exactly the partitions whose only missing home is slot 255 (the broker there leaves every row that
+      holds it as a non-leading home replica, for a broker no home list of that row names), DL is empty;
+    - "dl255": DL is exactly the partitions whose home0 is slot 255 (each led from another of its replicas).
+    Each list is checked with home_lists, so an edit to the construction cannot quietly empty it.  -> {name: base}"""
+    b255 = int(np.flatnonzero(slots(pb) == 255)[0])
+    D0, DL0 = home_lists(pb, reps)
+    assert DL0 == [] and all(set(int(b) for b in pb.cur[p][:4] if 0 <= b < pb.B) - set(reps[p]) == {b255} for p in D0)
+    out = {}
+    d = reps.copy()
+    for p in range(pb.P):
+        row = list(d[p])
+        if b255 in row[1:]:
+            home = set(int(b) for b in pb.cur[p][:4])
+            row[row.index(b255)] = next(b for b in range(pb.B) if b not in home and b not in row)
+            d[p] = row
+    D, DL = home_lists(pb, d)
+    assert len(D) >= 3 and DL == [], (len(D), DL)
+    assert all({int(b) for b in pb.cur[p][:4] if 0 <= b < pb.B} - set(d[p]) == {b255} for p in D)
+    out["d255"] = d
+    led = reps.copy()
+    for p in range(pb.P):
+        n = int((led[p] >= 0).sum())
+        if int(pb.cur[p][0]) == b255 and led[p][0] == b255 and n > 1:
+            led[p][:n] = np.roll(led[p][:n], -1)
+    D, DL = home_lists(pb, led)
+    want = [p for p in range(pb.P) if int(pb.cur[p][0]) == b255 and b255 in led[p] and led[p][0] != b255]
+    if want:
+        assert DL == want and D == D0, (DL, want)
+        out["dl255"] = led
+    return out

@@ -18,7 +18,7 @@ SHAPES = {
     "p8161_w1": lambda: m.synthetic_problem(8161, 32, 4, 3, remove=1),                       # 32 slots, one word
     "p65280_w2": lambda: m.synthetic_problem(65280, 64, 8, 3, remove=1),                     # 64 slots, 8 racks
     "p20000_w4": lambda: make_problem(20000, [20, 20, 20], 3, seed=41, removed=2),           # 3 racks of 20: padding slots
-    # 16 racks of up to 16: slot 255 stays padding (DESIGN.md 7.1: a home replica there reads as "no home slot")
+    # 16 racks of up to 16: slot 255 stays padding
     "p12000_w8": lambda: make_problem(12000, [16] * 15 + [15], 3, seed=42, removed=2),
     "p9000_dense": lambda: with_dense_weights(m.synthetic_problem(9000, 32, 4, 3, remove=1), 43),
 }

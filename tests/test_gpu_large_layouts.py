@@ -74,19 +74,6 @@ def empty_rows(reps):
     return int((reps < 0).all(1).sum())
 
 
-def skip_home_on_slot_255(pb):
-    """DESIGN.md 7.1's known limit, shared by every path: a home replica on slot 255 reads as "no home slot" to the
-    guided operations, while the restatement counts it (w8_s16 has one)"""
-    size = np.bincount(pb.rack_of, minlength=pb.R)
-    S = 8
-    while S < size.max():
-        S <<= 1
-    rank = np.array([int((pb.rack_of[:b] == pb.rack_of[b]).sum()) for b in range(pb.B)])
-    slot = pb.rack_of.astype(int) * S + rank                  # docs/MODEL.md §2: rack-major slots
-    if (slot[pb.cur[pb.cur >= 0]] == 255).any():
-        pytest.skip("a home replica on slot 255 (DESIGN.md 7.1)")
-
-
 # ---- every small layout through the HBM kernels ----------------------------------------------------------------
 @pytest.mark.parametrize("name", sorted(SMALL))
 def test_hbm_keys_and_evaluations_from_every_base(ref_lib, name):
@@ -95,7 +82,6 @@ def test_hbm_keys_and_evaluations_from_every_base(ref_lib, name):
     equals the model on random, short-row, duplicate-broker and emptied assignments."""
     pb = SMALL[name]()
     r = ref_lib.Ref(pb)
-    skip_home_on_slot_255(pb)
     sess = hbm_session(pb)
     lib = kopt.load_library()
     assert lib.kao_set_evaluator(sess._h, C.c_int32(0)) == -1 and "topic rows" in lib.kao_last_error().decode()
@@ -148,7 +134,6 @@ def test_hbm_long_walks_from_every_base(ref_lib, name):
     it does not hold in every round (an empty row is never refilled): the generator reads leader bytes throughout."""
     pb = SMALL[name]()
     r = ref_lib.Ref(pb)
-    skip_home_on_slot_255(pb)
     size = 256 if name in ROUND else 1024
     reps = r.decode(*r.init_base())
     for what, start in (("initial", reps), ("emptied", emptied_base(pb, reps, 5)), ("moved", moved_base(pb, reps, 6))):

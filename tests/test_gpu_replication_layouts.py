@@ -11,8 +11,7 @@ import rf_ref
 from oracle import model as m
 from problems import (C7_SHAPES, LARGE_SHAPES, LAYOUT_SHAPES, SHAPES, emptied_base, mixed_rows, moved_base,
                       off_rf_base)
-from test_gpu_large_layouts import (WALK, assert_keys, check_delta_keys, concentrated, empty_rows, malformed,
-                                    skip_home_on_slot_255)
+from test_gpu_large_layouts import WALK, assert_keys, check_delta_keys, concentrated, empty_rows, malformed
 
 pytestmark = pytest.mark.gpu
 
@@ -42,7 +41,6 @@ def test_replication_keys_and_evaluations_from_every_base(name):
     """Delta keys equal the restatement's from the initial, a random, an off-rf, an emptied and a moved base; get_base
     after set_base equals the model on random, short-row, duplicate-broker and emptied assignments."""
     pb = SMALL[name]()
-    skip_home_on_slot_255(pb)
     kp, tr, r = with_rows(pb)
     sess = kao.Session(kp)
     assert sess.stats()["words_per_row"] == r.W
@@ -94,7 +92,6 @@ def test_replication_long_walks_from_every_base(name):
     """48 rounds from the initial, an emptied and a moved base, without and (on a subset) with topic rows"""
     base_name = name.split("+")[0]
     pb = SMALL[base_name]()
-    skip_home_on_slot_255(pb)
     kp, tr, r = with_rows(pb, topics=name.endswith("+topics"))
     size = 256 if base_name in ROUND else 1024
     reps = r.decode(*r.init_base())

@@ -18,7 +18,7 @@ from kafka_assignment_optimizer_b200 import tuning
 from oracle import model as m
 from oracle import ref as oracle_ref
 from problems import C7_SHAPES, LAYOUT_SHAPES, SHAPES, emptied_base, moved_base, with_saturating_violation
-from test_gpu_large_layouts import assert_keys, empty_rows, skip_home_on_slot_255
+from test_gpu_large_layouts import assert_keys, empty_rows
 from test_gpu_layout_matrix import saturated_problem
 
 pytestmark = pytest.mark.gpu
@@ -108,7 +108,6 @@ def check_base(sess, pb, r, bits, ld, what):
 def test_long_and_probe_walks_from_every_base(ref_lib, name):
     pb = ALL[name]()
     assert pb.P <= 8160
-    skip_home_on_slot_255(pb)                       # w8_s16: its probe walk reaches the limit at round 107
     r = ref_lib.Ref(pb)
     run = runners(pb)
     size, ksize = ROUND.get(name, 1024), KEYS.get(name, 4096)

@@ -15,23 +15,12 @@ import kafka_assignment_optimizer_b200 as kao
 import topics_ref
 from emu import EmuSession
 from oracle import model as m
-from problems import (C7_SHAPES, LARGE_SHAPES, LAYOUT_SHAPES, LEADER255_SHAPES, SHAPES, SLOT255_SHAPES,
-                      SLOT255_TOPIC_SHAPES, emptied_base, moved_base)
-from test_gpu_large_layouts import skip_home_on_slot_255
+from problems import (C7_SHAPES, HOME255_SHAPES, LARGE_SHAPES, LAYOUT_SHAPES, LEADER255_SHAPES, SHAPES, SLOT255_SHAPES,
+                      SLOT255_TOPIC_SHAPES, emptied_base, home255_bases, moved_base, slots)
 from test_topics_cpu import interleaved_topics, sixteen_topics
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EVERY = {**SHAPES, **LAYOUT_SHAPES, **C7_SHAPES, **LARGE_SHAPES, **SLOT255_SHAPES, **LEADER255_SHAPES}
-
-
-def slots(pb):
-    """docs/MODEL.md §2: rack-major slots, S = pow2 >= max(8, largest rack) -> slot of every broker"""
-    size = np.bincount(pb.rack_of, minlength=pb.R)
-    S = 8
-    while S < size.max():
-        S <<= 1
-    rank = np.array([int((pb.rack_of[:b] == pb.rack_of[b]).sum()) for b in range(pb.B)])
-    return pb.rack_of.astype(int) * S + rank
+EVERY = {**SHAPES, **LAYOUT_SHAPES, **C7_SHAPES, **LARGE_SHAPES, **SLOT255_SHAPES, **LEADER255_SHAPES, **HOME255_SHAPES}
 
 
 def model4_initial_base(pb):
@@ -121,17 +110,22 @@ def test_golden_streams_are_what_the_restatement_computes(ref_lib):
         assert json.loads(json.dumps(mg.streams())) == json.load(f)
 
 
-def test_slot255_shapes_are_never_skipped():
-    """Every walk shape uses all 256 slots with broker 255 on slot 255 and no home replica there, so the known-limit
-    skip of the GPU tests (DESIGN.md 7.1) can never drop one silently; the initial-base shapes do lead from slot 255"""
-    for name, f in {**SLOT255_SHAPES, **SLOT255_TOPIC_SHAPES}.items():
+def test_slot255_shapes_are_never_skipped(ref_lib):
+    """Every 256-slot shape puts broker 255 on slot 255.  The grown-by-one walk shapes leave it empty; the home-255
+    shapes give it home replicas, and the initial base of each has targeted bases whose displaced lists are made of
+    home-255 partitions only (problems.home255_bases checks them); the initial-base shapes lead from slot 255."""
+    for name, f in {**SLOT255_SHAPES, **SLOT255_TOPIC_SHAPES, **HOME255_SHAPES}.items():
         pb = f()
         slot = slots(pb)
         assert pb.B == 256 and sorted(slot) == list(range(256)) and slot[255] == 255, name
-        try:
-            skip_home_on_slot_255(pb)
-        except pytest.skip.Exception:
-            pytest.fail("%s has a home replica on slot 255" % name)
+        on_255 = (slot[pb.cur[(pb.cur >= 0) & (pb.cur < pb.B)]] == 255).sum()
+        assert (on_255 > 0) == (name in HOME255_SHAPES), name
+    for name, f in HOME255_SHAPES.items():
+        pb = f()
+        r = ref_lib.Ref(pb)
+        assert r.W == 8, name
+        got = home255_bases(pb, r.decode(*r.init_base()))
+        assert set(got) == ({"d255"} if name == "h255_rf_down" else {"d255", "dl255"}), name
     for name, f in LEADER255_SHAPES.items():
         pb = f()
         assert slots(pb)[255] == 255 and (slots(pb)[pb.cur[:, 0][pb.cur[:, 0] >= 0]] == 255).any(), name

@@ -239,13 +239,15 @@ def _check_pins(select):
 def test_plain_and_replication_kernels_keep_their_pinned_sass():
     """Every kernel of the large-path and engine objects other than the topic search kernels as the build before the
     topic rows made it: neither the topic rows, the per-partition rows nor the topic functions in kao_topics.cuh
-    changed any of them."""
+    changed any of them.  The eight-word ones are pinned as the build that reads the home validity nibbles made them
+    (kao_device.cuh, home_valid: a home replica on slot 255 counts); the others never read them."""
     assert _check_pins(lambda name: not _TOPIC_SEARCH.search(name)) == 29
 
 
 def test_topic_search_kernels_keep_their_pinned_sass():
     """The four topic search kernels (W = 1, 2, 4, 8) as the build that tells padding slots from broker slots by the
-    order index against B (kao_topics.cuh, broker_slot) made them: slot 255 is a broker when B = 256."""
+    order index against B (kao_topics.cuh, broker_slot) made them: slot 255 is a broker when B = 256.  W = 8 as the
+    build that also reads the home validity nibbles made it."""
     assert _check_pins(lambda name: bool(_TOPIC_SEARCH.search(name))) == 4
 
 
