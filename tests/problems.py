@@ -474,3 +474,77 @@ def home255_bases(pb, reps):
         assert DL == want and D == D0, (DL, want)
         out["dl255"] = led
     return out
+
+
+# ---- replication factors 5 to 8 and RF = B - 1 (docs/MODEL.md §1, §3.2, §4, §5) ------------------------------------
+# Every shape above has RF <= 4 (C7_SHAPES reach 5 and 6 at 50 partitions).  Here: bit 2 and bit 3 of RF (the row pass
+# compares bit-sliced counts with four slices of RF), shortfalls of 4 and more (the tensor-core shortfall planes), 8
+# and 9 term planes at default weights (RFcur + 1 of them), initial bases that complete rows by five replicas or drop
+# the tail, and RF = B - 1, where REPLACE has exactly one broker the row does not use.
+RF_SHAPES = {
+    "rf7_cm": lambda: make_problem(200, [8] * 8, 7, RFcur=3, seed=201, removed=2),        # column-major, C7 0..1
+    "rf7_cur7": lambda: make_problem(200, [8] * 8, 7, seed=202),                         # 8 term planes
+    "rf7_cur8": lambda: make_problem(200, [8] * 8, 7, RFcur=8, seed=203),                # 9 term planes: row-major
+    "rf8_r8": lambda: make_problem(150, [8] * 8, 8, seed=204),                           # C7 1..1
+    # RF 8 on the column-major evaluator: eight racks of eight with C7 0..1 (RF 8 is bit 3 of the row pass's count)
+    "rf8_cm": lambda: dataclasses.replace(make_problem(150, [8] * 8, 8, RFcur=3, seed=214, removed=2), ppr_lo=0),
+    "rf8_b9": lambda: make_problem(60, [9], 8, seed=205),                                # RF = B - 1, C7 8..8
+    "rf8_r3_b9": lambda: make_problem(80, [4, 3, 2], 8, RFcur=5, seed=206),              # RF = B - 1, C7 2..3
+    # RF = B - 1 = 2 with C7 1..1: every row needs the one broker of the second rack, so no base is feasible
+    "rf2_b3": lambda: make_problem(40, [2, 1], 2, seed=207),
+    "rf2_b3_r3": lambda: make_problem(40, [1, 1, 1], 2, seed=207),                       # RF = B - 1, column-major
+    "rf8_w8": lambda: make_problem(120, [14] * 16, 8, seed=208, removed=3),              # 16-slot racks, W 8
+    "rf5_w8": lambda: make_problem(120, [20] * 6, 5, seed=209, removed=2),               # 32-slot racks, W 8
+    # 520 x RF 8 (P RF >= 4,096): the widest weights fit 12 bits, four current replicas keep packed entries
+    "rf8_w12": lambda: with_widest_cost_field(make_problem(520, [8] * 8, 8, RFcur=4, seed=210), 210),
+    "big_rf8": lambda: make_problem(8300, [8] * 8, 8, RFcur=3, seed=211),                # the HBM path
+    "big_rf8_b9": lambda: make_problem(8300, [9], 8, seed=212),                          # the HBM path, RF = B - 1
+}
+# small enough for HiGHS (oracle/model.py solve_exact), and feasible: RF = B - 1 at both ends, RF 8 over 10 brokers.
+# rf2_b3 is not among them: its C7 rows put every partition on the one broker of the second rack.
+RF_EXACT_SHAPES = {
+    "rf8_b9_p12": lambda: make_problem(12, [9], 8, seed=205),
+    "rf2_b3_r3": RF_SHAPES["rf2_b3_r3"],
+    "rf8_b10": lambda: make_problem(16, [5, 5], 8, seed=213),
+}
+
+
+def term_planes(pb):
+    """docs/MODEL.md §3.2 written out: the term planes of an objective, one per (kind, value) class times the largest
+    number of terms one partition has in it (kind F: wF, kind L: the bonus wL - wF); None if some wL < wF"""
+    most = {}
+    for p in range(pb.P):
+        n = {}
+        for b in np.flatnonzero(pb.wF[p] | pb.wL[p]):
+            f, l = int(pb.wF[p, b]), int(pb.wL[p, b])
+            if l < f:
+                return None
+            for cls in ((0, f), (1, l - f)):
+                if cls[1]:
+                    n[cls] = n.get(cls, 0) + 1
+        for cls, k in n.items():
+            most[cls] = max(most.get(cls, 0), k)
+    return sum(most.values())
+
+
+def one_per_rack_base(pb):
+    """Rows of RF replicas in RF distinct racks (RF <= R): partition p takes racks p, p + 1, .. (mod R), in each the
+    (p // R)-th broker (mod its size), leader first.  With C7 0..1 every row is well formed."""
+    members = [np.flatnonzero(pb.rack_of == r) for r in range(pb.R)]
+    out = np.empty((pb.P, pb.RF), np.int32)
+    for p in range(pb.P):
+        for k in range(pb.RF):
+            rack = members[(p + k) % pb.R]
+            out[p, k] = rack[(p // pb.R) % rack.size]
+    return out
+
+
+def reordered_base(reps):
+    """Every row of `reps` with its replicas in another order: row p rotated by 1 + p mod (n - 1), n its replicas, so
+    that another replica leads every row of two or more"""
+    out = reps.copy()
+    for p in range(out.shape[0]):
+        n = int((out[p] >= 0).sum())
+        if n > 1:
+            out[p, :n] = np.roll(out[p, :n], -(1 + p % (n - 1)))
+    return out
