@@ -601,13 +601,15 @@ uint64_t kao_ref_search(const ref_problem *pb, uint32_t *bits, uint8_t *leader, 
     const size_t nb = (size_t)pb->P * L.W;
     uint64_t last = KEY_NONE;
     uint64_t *keys = (uint64_t *)malloc((size_t)round_size * 8);
-    for (uint32_t t = first_round; t < first_round + rounds; ++t) {
+    /* round numbers are u32: call i runs round first_round + i mod 2^32 (docs/MODEL.md §6) */
+    for (uint32_t i = 0; i < rounds; ++i) {
+        const uint32_t t = first_round + i;
         uint64_t best = KEY_NONE;
         kao_ref_candidate_keys(pb, bits, leader, seed, t, round_size, 0, round_size, keys, nthreads);
-        for (uint32_t i = 0; i < round_size; ++i) if (keys[i] < best) best = keys[i];
+        for (uint32_t j = 0; j < round_size; ++j) if (keys[j] < best) best = keys[j];
         uint32_t widx = (uint32_t)(best & ((1u << IDX_BITS) - 1));
         kao_ref_gen(pb, bits, leader, seed, t, widx, round_size, bits, leader);
-        if (round_keys) round_keys[t - first_round] = best;
+        if (round_keys) round_keys[i] = best;
         last = best;
     }
     free(keys);

@@ -548,3 +548,75 @@ def reordered_base(reps):
         if n > 1:
             out[p, :n] = np.roll(out[p, :n], -(1 + p % (n - 1)))
     return out
+
+
+# ---- 64-bit seeds and late round numbers (docs/MODEL.md §5, §6) ----------------------------------------------------
+# A candidate is a function of (base, seed, round, idx): the seed is Philox's 64-bit key, the round number its u32
+# counter word 1, and every fourth round (round mod 4 = 3) a cycle round.  Seeds whose high word is set and round
+# numbers at and above 2^16, 2^24 and 2^31, and calls that cross 2^32 (rounds first_round + i mod 2^32).
+PHI = 0x9E3779B97F4A7C15            # kao_solve: restart r searches with seed + r * PHI mod 2^64
+SEEDS = {
+    "zero": 0,
+    "2^32": 1 << 32,                                # low word 0, high word 1
+    "high_word": 0xFFFFFFFF00000000,
+    "all_ones": (1 << 64) - 1,
+    "restart1_of_0": PHI,
+    "goldens_low": 0xDEADBEEF00C0FFEE,              # low word 0xC0FFEE, the goldens' seed
+}
+# first rounds: free (round mod 4 != 3) and cycle rounds; 2^32 - 2 with a walk of more than two rounds crosses 2^32
+ROUNDS = {
+    "3": 3,
+    "2^16-1": (1 << 16) - 1,
+    "2^16": 1 << 16,
+    "2^24-1": (1 << 24) - 1,
+    "2^24": 1 << 24,
+    "2^31+3": (1 << 31) + 3,
+    "2^32-2": (1 << 32) - 2,
+}
+WRAP = ROUNDS["2^32-2"]
+
+
+def round_at(first, i):
+    """round i of a call that starts at `first` (docs/MODEL.md §6)"""
+    return (first + i) % (1 << 32)
+
+
+def patience_stop(keys, n):
+    """The kernel's rule: stop after n rounds in a row whose (violation, cost) is not strictly better than the best so
+    far -> rounds run"""
+    best, stall = None, 0
+    for t, k in enumerate(keys):
+        vc = int(k) >> 24
+        if best is None or vc < best:
+            best, stall = vc, 0
+        else:
+            stall += 1
+        if stall >= n:
+            return t + 1
+    return len(keys)
+
+
+def ref_solve(r, seed, restarts, rounds, size, patience=0, chunk=100):
+    """kao_solve restated over a restatement `r` (oracle/ref.py Ref, TRef, RRef): restart k resets to the initial base
+    and searches with seed + k * PHI mod 2^64 from round 0 (stopping where patience says); the best final base by
+    (violation, -objective) wins, the lowest restart on a tie.  -> dict(violation, objective, replicas, key, rounds
+    (summed over the restarts), restart)"""
+    best, total = None, 0
+    for k in range(restarts):
+        s = (seed + k * PHI) % (1 << 64)
+        n = rounds
+        if patience:
+            bits, ld = r.init_base()
+            keys = []
+            while len(keys) < rounds and patience_stop(keys, patience) == len(keys):
+                keys += list(r.search(bits, ld, s, len(keys), min(chunk, rounds - len(keys)), size)[1])
+            n = patience_stop(keys, patience)
+        bits, ld = r.init_base()
+        _, keys = r.search(bits, ld, s, 0, n, size)
+        total += n
+        v, o = r.evaluate(bits, ld)
+        if best is None or (v, -o) < (best["violation"], -best["objective"]):
+            best = dict(violation=v, objective=o, replicas=r.decode(bits, ld), restart=k,
+                        key=int(keys[-1]) if n else 0x7FFFFFFFFFFFFFFF)
+    best["rounds"] = total
+    return best

@@ -17,7 +17,8 @@ from kafka_assignment_optimizer_b200 import optimizer as kopt
 from kafka_assignment_optimizer_b200 import tuning
 from oracle import model as m
 from oracle import ref as oracle_ref
-from problems import C7_SHAPES, LAYOUT_SHAPES, SHAPES, emptied_base, moved_base, with_saturating_violation
+from problems import (C7_SHAPES, LAYOUT_SHAPES, SHAPES, emptied_base, moved_base, patience_stop,
+                      with_saturating_violation)
 from test_gpu_large_layouts import assert_keys, empty_rows
 from test_gpu_layout_matrix import saturated_problem
 
@@ -210,21 +211,6 @@ def test_entry_points_in_turn_on_one_session(ref_lib, name, base):
 
 
 # ---- patience against its definition -------------------------------------------------------------------------------
-def patience_stop(keys, n):
-    """The kernel's rule: stop after n rounds in a row whose (violation, cost) is not strictly better than the best so
-    far -> rounds run"""
-    best, stall = None, 0
-    for t, k in enumerate(keys):
-        vc = int(k) >> 24
-        if best is None or vc < best:
-            best, stall = vc, 0
-        else:
-            stall += 1
-        if stall >= n:
-            return t + 1
-    return len(keys)
-
-
 def restatement_until_stop(r, bits, ld, seed, n, cap, size, chunk=100):
     keys = np.zeros(0, np.uint64)
     while len(keys) < cap:

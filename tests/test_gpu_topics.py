@@ -11,7 +11,7 @@ import kafka_assignment_optimizer_b200 as kao
 import topics_ref
 from kafka_assignment_optimizer_b200 import optimizer as kopt
 from oracle import model as m
-from problems import with_dense_weights
+from problems import ref_solve, with_dense_weights
 from conftest import make_problem
 
 pytestmark = pytest.mark.gpu
@@ -124,29 +124,19 @@ def test_non_binding_topic_rows_leave_the_delta_solve_as_it_is(name):
     assert (loose.replicas == plain.replicas).all()
 
 
-def _ref_solve(r, seed, restarts, rounds, size):
-    best = None
-    for k in range(restarts):
-        bits, ld = r.init_base()
-        r.search(bits, ld, (seed + 0x9E3779B97F4A7C15 * k) % 2 ** 64, 0, rounds, size)
-        v, o = r.evaluate(bits, ld)
-        if best is None or (v, -o) < (best[0], -best[1]):
-            best = (v, o, r.decode(bits, ld))
-    return best
-
-
 @pytest.mark.parametrize("spread", [False, True])
 def test_topic_solve_with_restarts_equals_the_restatement(ref_lib, spread):
     import torch
 
     pb, tr = SHAPES["p700_w1_t30"]()
     r = topics_ref.TRef(pb, tr)
-    v, o, reps = _ref_solve(r, 0xC0FFEE, 3, 6, 2048)
+    want = ref_solve(r, 0xC0FFEE, 3, 6, 2048)
     n = torch.cuda.device_count() if spread else 1
     res = kopt.solve(kao.Problem.from_fields(pb), seed=0xC0FFEE, rounds=6, round_size=2048, restarts=3,
                      spread_restarts=spread, n_gpus=n, topic_balance=True)
-    assert (res.violation, res.objective) == (v, o) and (res.replicas == reps).all()
-    assert res.rounds == 18
+    assert (res.violation, res.objective) == (want["violation"], want["objective"])
+    assert (res.replicas == want["replicas"]).all() and res.key == want["key"]
+    assert res.rounds == want["rounds"] == 18
 
 
 def readme_three_topics():

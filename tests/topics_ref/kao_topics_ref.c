@@ -88,12 +88,13 @@ uint64_t kao_tref_search(const ref_problem *pb, const ref_topics *tp, uint32_t *
 {
     uint64_t last = KEY_NONE;
     uint64_t *keys = (uint64_t *)malloc((size_t)round_size * 8);
-    for (uint32_t t = first_round; t < first_round + rounds; ++t) {
+    for (uint32_t i = 0; i < rounds; ++i) {                 /* round first_round + i mod 2^32 (docs/MODEL.md §6) */
+        const uint32_t t = first_round + i;
         uint64_t best = KEY_NONE;
         kao_tref_candidate_keys(pb, tp, bits, leader, seed, t, round_size, 0, round_size, keys, nthreads);
-        for (uint32_t i = 0; i < round_size; ++i) if (keys[i] < best) best = keys[i];
+        for (uint32_t j = 0; j < round_size; ++j) if (keys[j] < best) best = keys[j];
         kao_ref_gen(pb, bits, leader, seed, t, (uint32_t)(best & ((1u << IDX_BITS) - 1)), round_size, bits, leader);
-        if (round_keys) round_keys[t - first_round] = best;
+        if (round_keys) round_keys[i] = best;
         last = best;
     }
     free(keys);
